@@ -1,5 +1,5 @@
 """Reference arm: drives the UNMODIFIED Samsung/veles.znicz CIFAR-10 sample
-(``baseline/_ref/veles/znicz/samples/CIFAR10/cifar.py`` + ``cifar_caffe_config.py``) through
+(``oracle/_ref/veles/znicz/samples/CIFAR10/cifar.py`` + ``cifar_caffe_config.py``) through
 its own public API — ``run(load, main)`` → ``CifarWorkflow`` (StandardWorkflow) →
 ``initialize(device)`` → ``run()`` — on the stock ``cuda_run`` path of its units (NVRTC build of
 its ``cuda/*.cu``, cuBLAS SGEMM). The absent Veles core / cuda4py / zope.interface are the shim
@@ -17,12 +17,13 @@ import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CORE = os.path.join(HERE, "veles_core")
-REF = os.path.join(HERE, "_ref", "veles", "znicz")
+ORACLE = os.path.join(os.path.dirname(HERE), "oracle")
+REF = os.path.join(ORACLE, "_ref", "veles", "znicz")
 
 
 def ensure_reference():
     if not os.path.isfile(os.path.join(REF, "MANIFEST.sha256.json")):
-        sys.path.insert(0, HERE)
+        sys.path.insert(0, ORACLE)
         import install_reference
         install_reference.install()
 

@@ -62,8 +62,8 @@ class Device(object):
         _init()
         self.index = index
         if DRY:
-            self.handle, self.name, self.compute_capability = None, "dry", (10, 0)
-            self.multiprocessor_count, self.total_mem = 148, 180 << 30
+            self.handle, self.name, self.compute_capability = None, "dry", (9, 0)
+            self.multiprocessor_count, self.total_mem = 132, 80 << 30
             return
         self.handle = _ck(_drv.cuDeviceGet(index))
         name = _ck(_drv.cuDeviceGetName(128, self.handle))
@@ -306,7 +306,7 @@ class Module(object):
                 source = f.read()
         if source is None:
             raise ValueError("source is required")
-        cc = context.device.compute_capability if context is not None else (10, 0)
+        cc = context.device.compute_capability if context is not None else (9, 0)
         self.binary = compile_source(source, include_dirs, options, cc)
         if context is not None and not DRY:
             context.set_current()
@@ -320,7 +320,7 @@ class Module(object):
     get_function = create_function
 
 
-def compile_source(source, include_dirs=(), options=(), cc=(10, 0), name="veles_program.cu"):
+def compile_source(source, include_dirs=(), options=(), cc=(9, 0), name="veles_program.cu"):
     """CUDA C -> cubin for sm_<cc> with NVRTC (works without a GPU)."""
     prog = _nck(_nvrtc.nvrtcCreateProgram(source.encode(), name.encode(), 0, [], []))
     opts = [("--gpu-architecture=sm_%d%d" % tuple(cc)).encode(), b"--std=c++14",

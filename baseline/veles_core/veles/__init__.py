@@ -5,7 +5,7 @@
 NVRTC program build, driver-API launches, cuBLAS GEMM, full-batch loaders.
 
 It exists ONLY so that ``bench.py --impl reference`` can run the UNMODIFIED reference
-units (``baseline/_ref/veles/znicz``) through their stock ``cuda_run`` path on a B200.
+units (``oracle/_ref/veles/znicz``) through their stock ``cuda_run`` path on an H100.
 Nothing of veles.znicz_b200 (the product) is imported here.
 """
 import importlib.abc
@@ -18,7 +18,8 @@ __root__ = os.path.dirname(os.path.abspath(__file__))
 __version__ = "0.0.shim"
 __plugins__ = set()
 
-_ref = os.path.join(os.path.dirname(os.path.dirname(__root__)), "_ref", "veles")
+_ref = os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(__root__))), "oracle", "_ref",
+                    "veles")
 if os.path.isdir(_ref):
     __path__.append(_ref)          # veles.znicz = the vendored, unmodified reference
 

@@ -6,7 +6,7 @@ consumed by the reference (e.g. /root/reference/samples/Wine/wine_config.py:43-5
 are plain python files doing ``root.<ns>.update({...})``; engine keys live under
 ``root.common.engine`` and directories under ``root.common.dirs``.
 
-Design notes (B200-first): the tree also carries the B200 engine switches
+Design notes (H100-first): the tree also carries the H100 engine switches
 (``root.common.engine.backend`` in {"numpy", "cuda"}, ``precision_type`` in
 {"float", "double", "bf16"}, ``graphs`` for CUDA-graph capture of the
 minibatch step).
@@ -140,7 +140,7 @@ def _defaults():
                           os.path.join(tempfile.gettempdir(), "veles_ref_shim"))
     root.common.update({
         "engine": {
-            # "numpy" (CPU oracle) or "cuda" (sm_100a). "auto" picks cuda when present.
+            # "numpy" (CPU oracle) or "cuda" (sm_90a). "auto" picks cuda when present.
             "backend": "auto",
             # host/master dtype: "float" | "double"; device compute dtype is
             # selected with compute_type: "fp32" | "bf16" | "fp8"

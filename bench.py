@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Flagship benchmark: CIFAR-10 caffe-conv training throughput (images/s, whole job).
 
-Contract (see the round brief): ``python bench.py --gpus N --steps K --warmup W`` (the
-driver launches it with torch.distributed.run for N > 1); rank 0 prints ONE JSON line.
+Usage: ``python bench.py --gpus N --steps K --warmup W`` (launched with torch.distributed.run
+for N > 1); rank 0 prints ONE JSON line. ``--dump-outputs DIR`` additionally writes what the timed
+path computed in its last step (see ``dump_outputs``).
 
 * model/config: /root/reference/samples/CIFAR10/cifar_caffe_config.py:52-145 — conv32-5p2 /
   maxpool3s2 / relu / LRN / conv32-5p2 / relu / avgpool3s2 / LRN / conv64-5p2 / relu / avgpool3s2 /
@@ -149,6 +150,50 @@ def _batch_of(model):
     return int(os.environ.get("ZNICZ_BENCH_BATCH", MODELS[model][0]))
 
 
+DUMP_BUDGET = 64 << 20            # bytes of .npy payload written by --dump-outputs, at most
+DUMP_MAX_ELEMS = 1 << 19          # larger arrays: a fixed, seeded sample of this many elements
+
+
+def dump_outputs(wf, out_dir):
+    """Write the arrays a caller of the timed training step receives after its last step: the
+    network output and the evaluator's results for that minibatch, and every layer's updated
+    weights and bias, as ``out_dir/<name>.npy`` (float32; integer results as float64). An array
+    larger than DUMP_MAX_ELEMS is replaced by a sorted sample of that many elements drawn with a
+    fixed seed (``<name>.sample.npy``), so that two builds can be compared output for output."""
+    import numpy
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = []
+    last = wf.forwards[-1]
+    arrays.append(("output", last.output))
+    for attr in ("err_output", "n_err", "max_err_output_sum", "confusion_matrix", "metrics"):
+        v = getattr(wf.evaluator, attr, None)
+        if v is not None and hasattr(v, "map_read"):
+            arrays.append(("evaluator_" + attr, v))
+    for i, u in enumerate(wf.forwards):
+        for attr in ("weights", "bias"):
+            v = getattr(u, attr, None)
+            if v is not None and hasattr(v, "map_read") and v:
+                arrays.append(("layer%02d_%s_%s" % (i, type(u).__name__, attr), v))
+    written, total = [], 0
+    for name, vec in arrays:
+        if not vec:
+            continue
+        vec.map_read()
+        a = numpy.asarray(vec.mem)
+        a = a.astype(numpy.float64 if a.dtype.kind in "iub" else numpy.float32)
+        a = numpy.ascontiguousarray(a)
+        if a.size > DUMP_MAX_ELEMS:
+            idx = numpy.sort(numpy.random.RandomState(1234).randint(0, a.size, DUMP_MAX_ELEMS))
+            a = a.reshape(-1)[idx]
+            name += ".sample"
+        if total + a.nbytes > DUMP_BUDGET:
+            break
+        numpy.save(os.path.join(out_dir, name + ".npy"), a)
+        total += a.nbytes
+        written.append(name)
+    return written
+
+
 def run_arm(args, streaming):
     import torch
     if os.environ.get("ZNICZ_OVERLAP_WGRAD") == "0":        # diagnostic
@@ -202,11 +247,15 @@ def run_arm(args, streaming):
     launches0 = api.counters["launches"]
     t0 = time.perf_counter()
     e0.record()
-    wf.run(iterations=args.steps)
+    n_steps = wf.run(iterations=args.steps)
     e1.record()
     t_enq = time.perf_counter()       # host finished enqueueing (the device may still be busy)
     torch.cuda.synchronize()
     t1 = time.perf_counter()
+    if n_steps != args.steps:
+        raise RuntimeError("the timed loop ran %d steps, not --steps %d" % (n_steps, args.steps))
+    if args.dump_outputs and not streaming and int(os.environ.get("RANK", "0")) == 0:
+        dump_outputs(wf, args.dump_outputs)
     if world > 1:
         dist.barrier()
     clocks = sampler.stop()
@@ -307,7 +356,7 @@ def _reference_timed(args, rank, world, streaming):
 
 
 def run_reference_arm(args, rank, world):
-    """``--impl reference``: the UNMODIFIED reference (baseline/_ref) on its own stock GPU path;
+    """``--impl reference``: the UNMODIFIED reference (oracle/_ref) on its own stock GPU path;
     the product package is never imported in this process."""
     try:
         if not os.environ.get("CUDA4PY_DRY"):
@@ -349,7 +398,7 @@ def run_reference_arm(args, rank, world):
                    "%d independent replicas, no parameter exchange (upper bound of the "
                    "reference's asynchronous master/slave scheme, whose ZeroMQ/Twisted "
                    "transport lives in the absent Veles core)" % n,
-                   "code": "unmodified Samsung/veles.znicz (baseline/_ref, sha256 manifest): "
+                   "code": "unmodified Samsung/veles.znicz (oracle/_ref, sha256 manifest): "
                            "samples/CIFAR10/cifar.py + cifar_caffe_config.py, stock cuda_run "
                            "path (NVRTC build of its cuda/*.cu + cuBLAS SGEMM, precision_type "
                            "float)",
@@ -390,7 +439,14 @@ def main():
                          "of the per-GPU batch of the config")
     ap.add_argument("--model", default="cifar_caffe", choices=sorted(MODELS),
                     help="cifar_caffe is the north-star config; the others are extra data points")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the device-timed steps (the reported value; not the end-to-end "
+                         "streaming loop) write the last step's outputs (network output, evaluator "
+                         "results, updated weights) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs is not supported with --impl reference (the reference arm runs "
+                 "the unmodified reference, whose arrays this script does not export)")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.impl == "reference":

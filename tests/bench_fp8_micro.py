@@ -1,5 +1,5 @@
-"""bf16 vs fp8 (e4m3) tcgen05 GEMM on FC-shaped problems (CUDA events, L2 flushed between
-launches). Run on a B200:  python tests/bench_fp8_micro.py"""
+"""bf16 vs fp8 (e4m3) wgmma GEMM on FC-shaped problems (CUDA events, L2 flushed between
+launches). Run on an H100:  python tests/bench_fp8_micro.py"""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""Numerics + throughput of the 2-CTA persistent tcgen05 GEMM (csrc/gemm_pair.cu) against the
+"""Numerics + throughput of the persistent warp-specialised wgmma GEMM (csrc/gemm_pair.cu) against the
 single-CTA kernel (gemm_umma.cu) and cuBLAS (torch.matmul), same process, CUDA events, L2 flushed
 between timed launches. usage: python tests/bench_gemm_pair.py [check|bench]"""
 import json

@@ -1,5 +1,5 @@
 """H2D copy timing from pinned memory (CUDA events), alone and queued behind a kernel.
-Run on a B200:  python tests/bench_h2d_micro.py"""
+Run on an H100:  python tests/bench_h2d_micro.py"""
 import torch
 
 dev = "cuda"

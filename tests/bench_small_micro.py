@@ -1,6 +1,6 @@
 """Micro-benchmark of the latency-bound (tiny batch) GEMM / conv launches of the GA-tuned MNIST
 conv net (batch 6). CUDA events; each shape timed with a cold L2 (256 MB write between launches)
-and warm (back-to-back launches). Run on a B200:  python tests/bench_small_micro.py
+and warm (back-to-back launches). Run on an H100:  python tests/bench_small_micro.py
 """
 import os
 import sys

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a real B200 (run by gpurun)")
+    config.addinivalue_line("markers", "gpu: test needs an H100 GPU")
     config.addinivalue_line("markers", "slow: long-running test")
 
 

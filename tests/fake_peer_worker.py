@@ -85,7 +85,8 @@ def main():
     gss = [torch.zeros(2, dtype=torch.int32, device=dev) for _ in range(N)]
     streams = [torch.cuda.Stream() for _ in range(N)]
     torch.cuda.synchronize()
-    cap = MAX_BLOCKS // N
+    # all N launches must be co-resident: 4 CTAs per SM between them
+    cap = min(MAX_BLOCKS, 4 * torch.cuda.get_device_properties(dev).multi_processor_count) // N
     for _step in range(3):
         for r in range(N):
             with torch.cuda.stream(streams[r]):

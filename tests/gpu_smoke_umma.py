@@ -1,4 +1,4 @@
-"""Stand-alone first-contact check of the tcgen05 kernels (run under `timeout`):
+"""Stand-alone first-contact check of the wgmma kernels (run under `timeout`):
 prints per-configuration max relative error so a descriptor mistake is visible at once."""
 import sys
 import os

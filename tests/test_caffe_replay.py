@@ -1,9 +1,9 @@
-"""Whole-iteration replay of a Caffe CIFAR-10 training step, layer by layer
-(/root/reference/tests/functional/test_caffe_complex.py:83-534 on
-``data/cifar_export.tar.xz``; iteration 0 converted by tools/make_caffe_replay.py into
-tests/data/caffe_cifar_iter0.npz, batch 3): every layer gets Caffe's bottom blob / weights /
-top gradient and must reproduce Caffe's top blob / bottom gradient - on the numpy oracle
-(CPU tier) and on the sm_100a path in fp32 and bf16 (GPU tier)."""
+"""Whole-iteration replay of a Caffe CIFAR-10 training step, layer by layer (the reference's
+tests/functional/test_caffe_complex.py:83-534 on its ``data/cifar_export.tar.xz``; iteration 0,
+batch 3, converted by tools/make_caffe_replay.py into tests/golden/caffe_replay/): every layer gets
+Caffe's bottom blob / weights / top gradient and must reproduce Caffe's top blob / bottom gradient -
+on the numpy oracle (CPU tier) and on the sm_90a path in fp32 and bf16 (GPU tier)."""
+import glob
 import os
 
 import numpy
@@ -15,9 +15,26 @@ from veles.znicz_b200.core.workflow import DummyWorkflow
 from veles.znicz_b200.ops import (activation, all2all, conv, gd, gd_conv, gd_pooling,
                                   normalization, pooling)
 
-NPZ = os.path.join(os.path.dirname(os.path.abspath(__file__)), "data", "caffe_cifar_iter0.npz")
-D = numpy.load(NPZ) if os.path.isfile(NPZ) else None
-pytestmark = pytest.mark.skipif(D is None, reason="tests/data/caffe_cifar_iter0.npz missing")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "caffe_replay")
+
+
+def _load():
+    """{blob name: array} of iteration 0; names listed in ``__aliases__`` share a stored blob."""
+    blobs, aliases = {}, []
+    for path in sorted(glob.glob(os.path.join(GOLDEN, "iter0_*.npz"))):
+        with numpy.load(path) as z:
+            for k in z.files:
+                if k == "__aliases__":
+                    aliases += [str(x) for x in z[k]]
+                else:
+                    blobs[k] = z[k]
+    for a in aliases:
+        name, stored = a.split("=")
+        blobs[name] = blobs[stored]
+    return blobs
+
+
+D = _load()
 
 CONVS = {"conv1": 32, "conv2": 32, "conv3": 64}
 POOLS = {"pool1": pooling.MaxPooling, "pool2": pooling.AvgPooling, "pool3": pooling.AvgPooling}
@@ -31,7 +48,8 @@ def _rel(a, b):
 
 
 def _arr(x, device, compute):
-    a = Array(numpy.ascontiguousarray(x, dtype=numpy.float32))
+    # a copy: aliased blobs share one stored array, which no unit may write into
+    a = Array(numpy.array(x, dtype=numpy.float32, order="C"))
     if device is not None and compute == "bf16":
         import torch
         a.dev_dtype = torch.bfloat16

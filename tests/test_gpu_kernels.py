@@ -1,4 +1,4 @@
-"""Direct numerics tests of the sm_100a kernels against plain PyTorch fp32 references."""
+"""Direct numerics tests of the sm_90a kernels against plain PyTorch fp32 references."""
 import numpy
 import pytest
 import torch
@@ -104,7 +104,7 @@ CONV_CASES = [
     (3, 14, 17, 64, 64, 3, 5, (2, 1, 1, 0), (1, 1)),    # asymmetric padding, tiles span images
     (2, 16, 16, 64, 64, 3, 3, (1, 1, 1, 1), (2, 2)),    # strided windows (dgrad stays on gather)
     (5, 13, 13, 192, 128, 3, 3, (1, 1, 1, 1), (1, 1)),  # AlexNet conv3-like, 3 channel slices / tap
-    # large layers: 2-CTA persistent kernel (gemm_pair.cu) with the TMA im2col operand
+    # large layers: persistent kernel (gemm_pair.cu) with the TMA im2col operand
     (8, 13, 13, 128, 256, 3, 3, (1, 1, 1, 1), (1, 1)),  # fprop BN 256; dgrad N = 128
     (4, 20, 20, 64, 384, 5, 5, (2, 2, 2, 2), (1, 1)),   # fprop 3 N-tiles of 128
     (3, 20, 21, 256, 128, 3, 3, (1, 1, 1, 1), (1, 1)),  # dgrad BN 256, ragged M
@@ -507,7 +507,7 @@ def test_lrn_backward_with_producer_derivative(ext, dtype, c):
 @pytest.mark.parametrize("M,N,K", [(128, 256, 512), (100, 72, 384), (257, 1000, 4096)])
 @pytest.mark.parametrize("out_dt", [torch.bfloat16, torch.float32])
 def test_gemm_fp8_e4m3(ext, M, N, K, out_dt):
-    """tcgen05 kind::f8f6f4 GEMM on per-tensor-scaled e4m3 operands: exact (up to fp32
+    """wgmma e4m3 GEMM on per-tensor-scaled e4m3 operands: exact (up to fp32
     accumulation order) against the same quantised operands multiplied in fp32, and within
     fp8 tolerance of the unquantised product."""
     torch.manual_seed(M + N)
@@ -544,7 +544,7 @@ def test_gemm_fp8_e4m3(ext, M, N, K, out_dt):
                                            (768, 384, 200, False, 0), (512, 256, 128, True, 0),
                                            (2048, 4096, 1024, False, 0)])
 def test_gemm_pair_2cta_persistent(ext, M, N, K, f32, act):
-    """csrc/gemm_pair.cu (cta_group::2, persistent, TMEM double buffering, TMA store) vs fp32
+    """csrc/gemm_pair.cu (persistent, producer + two wgmma warpgroups, TMA store) vs fp32
     PyTorch, with the 2x-NaN out-of-bounds guard."""
     torch.manual_seed(M + N)
     dev = "cuda"
@@ -566,7 +566,7 @@ def test_gemm_pair_2cta_persistent(ext, M, N, K, f32, act):
 
 @pytest.mark.parametrize("batch,n_out,n_in", [(128, 512, 1024), (64, 1000, 768), (200, 256, 4104)])
 def test_fc_wgrad_pair(ext, batch, n_out, n_in):
-    """gradW[out][in] = err^T . x on the 2-CTA kernel (both operands MN-major, K = batch)."""
+    """gradW[out][in] = err^T . x on the persistent kernel (both operands MN-major, K = batch)."""
     torch.manual_seed(batch)
     dev = "cuda"
     err = torch.randn(batch, n_out, device=dev).bfloat16()

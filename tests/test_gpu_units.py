@@ -1,4 +1,4 @@
-"""numpy-oracle vs sm_100a path for every unit (oracle style (b) of SURVEY §4;
+"""numpy-oracle vs sm_90a path for every unit (oracle style (b) of SURVEY §4;
 /root/reference/tests/unit/test_all2all.py:138-152, test_gd.py:158-175), in fp32 and bf16,
 with the 2x-NaN out-of-bounds guard idea applied to device buffers."""
 import numpy
@@ -233,7 +233,7 @@ def test_lstm_sequence(compute, seq):
 @pytest.mark.parametrize("shape,hidden", [((40, 7, 64), 64), ((150, 5, 128), 256)])
 def test_lstm_persistent_kernels(seq, shape, hidden):
     """Whole-sequence cluster kernels (csrc/lstm_persist.cu: W resident in shared memory, gates GEMM
-    on tcgen05, cell math from TMEM, h exchanged through L2 under barrier.cluster) against the
+    on wgmma, cell math on the register accumulators, h exchanged through L2 under barrier.cluster) against the
     numpy oracle; batch 150 = two clusters with a ragged second tile; ZNICZ_LSTM_PERSIST=0 is the
     per-step path and must agree as well."""
     import os

@@ -1,5 +1,4 @@
-"""numpy oracle vs sm_100a path for the units round 1 left without a GPU test (VERDICT r1
-"unverified device paths"): Deconv / GDDeconv (tcgen05 kernels with swapped roles, alpha/beta,
+"""numpy oracle vs sm_90a path for the units not covered by test_gpu_units.py: Deconv / GDDeconv (wgmma kernels with swapped roles, alpha/beta,
 hits), Depooling, Kohonen SOM (forward + trainer, scalar and GEMM formulations), EvaluatorMSE
 (+ denormalisation + nearest class target), stochastic pool-depool, Cutter1D,
 Multiplier / Summator and their GD units."""
@@ -113,7 +112,7 @@ def test_depooling(compute):
 
 @pytest.mark.parametrize("neurons_shape,length", [((4, 4), 2), ((8, 8), 40), ((16, 12), 257)])
 def test_kohonen_forward_and_trainer(neurons_shape, length):
-    """Scalar kernels for tiny feature vectors, split-bf16 tcgen05 GEMM distances otherwise
+    """Scalar kernels for tiny feature vectors, split-bf16 wgmma GEMM distances otherwise
     (the reference computes the distances with its tiled matmul, /root/reference/ocl/kohonen.cl:19-36)."""
     rs = numpy.random.RandomState(8)
     data = rs.uniform(-1, 1, (96, length)).astype(numpy.float32)
@@ -237,7 +236,7 @@ def test_stochastic_pool_depool_gpu():
 
 def test_fp32_layers_run_on_tensor_cores():
     """compute_type fp32 (the reference's precision): FC and conv layers run as split-bf16
-    (hi/lo) tcgen05 GEMMs (kernels/fp32x.py) and still match the numpy oracle to fp32-like
+    (hi/lo) wgmma GEMMs (kernels/fp32x.py) and still match the numpy oracle to fp32-like
     accuracy - 600x tighter than the bf16 path's bound; the switch restores the SIMT kernels."""
     from test_gpu_units import _compare
     from veles.znicz_b200.kernels import fp32x

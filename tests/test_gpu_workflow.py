@@ -1,4 +1,4 @@
-"""End-to-end StandardWorkflow on a real B200: eager + CUDA-graph segments, fp32 + bf16."""
+"""End-to-end StandardWorkflow on a real H100: eager + CUDA-graph segments, fp32 + bf16."""
 import numpy
 import pytest
 
@@ -157,7 +157,7 @@ def test_fp32_tensor_core_training_matches_simt():
 def test_activation_fusion_equals_separate_units(compute, tol):
     """conv→relu / maxpool→relu / conv→relu folded into the producers' kernels (forward), the
     derivative folded into the pooling backward and - bf16 - the bias gradient delivered by the
-    tcgen05 wgrad kernel must train like the stand-alone units (eager)."""
+    wgmma wgrad kernel must train like the stand-alone units (eager)."""
     from veles.znicz_b200.core import prng
     results, counts = [], []
     for fuse in (False, True):

@@ -1,7 +1,7 @@
-"""Per-kernel SASS listings for profiles/sass/: one file per kernel family (first template
-instantiation of each, plus the named flagship instantiations), and an index with the
-Blackwell-relevant mnemonic counts of EVERY instantiation (UTC*MMA = tcgen05.mma, LDTM =
-tcgen05.ld, UTMALDG/UTMASTG = TMA, LDGMC = multimem.ld_reduce, HMMA would be the legacy path)."""
+"""Per-kernel SASS listings under profiles/sass/ (git-ignored): one file per kernel family (first
+template instantiation of each, plus the named flagship instantiations), and an index with the
+Hopper-relevant mnemonic counts of EVERY instantiation (HGMMA = wgmma, WARPGROUP = its
+fences, UTMALDG/UTMASTG = TMA, LDGMC = multimem.ld_reduce, HMMA would be the legacy path)."""
 import collections
 import os
 import re
@@ -11,7 +11,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "veles", "znicz_b200", "kernels", "_znicz_b200_C.so")
 OUT = os.path.join(ROOT, "profiles", "sass")
-MNEMONICS = ("UTCHMMA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "LDGSTS",
+MNEMONICS = ("HGMMA", "WARPGROUP", "USETMAXREG", "UTMALDG", "UTMASTG", "UBLKCP", "LDGSTS",
              "LDGMC", "STGMC", "REDGMC", "UCGABAR", "SYNCS", "HMMA", "FFMA", "MUFU", "ATOM", "RED.")
 KEEP_EXTRA = ("gemm_pair_k<256, false>", "gemm_pair_k<(int)256, (bool)0>")
 
@@ -53,12 +53,12 @@ def main():
             seen.setdefault(fam, fn)
             with open(os.path.join(OUT, fn + ".sass"), "w") as out:
                 out.write("// %s\n// (%d instructions; cuobjdump -sass of the in-tree "
-                          "_znicz_b200_C.so, sm_100a)\n" % (name, len(code)))
+                          "_znicz_b200_C.so, sm_90a)\n" % (name, len(code)))
                 # strip the encoding column: keeps the listing readable and ~3x smaller
                 for l in code:
                     out.write(re.sub(r"\s*/\* 0x[0-9a-f]+ \*/\s*$", "", l).rstrip() + "\n")
     with open(os.path.join(OUT, "INDEX.md"), "w") as out:
-        out.write("# SASS index (tools/dump_sass.py; sm_100a, %d kernels)\n\n" % len(index))
+        out.write("# SASS index (tools/dump_sass.py; sm_90a, %d kernels)\n\n" % len(index))
         out.write("| family | instantiation | instr | " + " | ".join(MNEMONICS) + " |\n")
         out.write("|---|---|---|" + "---|" * len(MNEMONICS) + "\n")
         for fam, name, n, c in sorted(index):

@@ -1,8 +1,12 @@
 """Converts ONE iteration of the reference's Caffe CIFAR export
 (/root/reference/tests/functional/data/cifar_export.tar.xz: text dumps of every layer's blobs
-before/after its forward and backward pass, batch 3) into a compact ``.npz`` that travels with
-the repo (the tarball is 65 MB of text and only exists where the reference is mounted).
-Arrays are NHWC float32; weights keep Caffe's [F][C][ky][kx] order."""
+before/after its forward and backward pass, batch 3) into the fixtures of
+tests/test_caffe_replay.py under ``tests/golden/caffe_replay/`` (the tarball is 65 MB of text and
+only exists where the reference is mounted). Only the blobs the replay compares are kept; a blob
+that Caffe dumps identically under several names (in-place layers, a layer's top = the next
+layer's bottom) is stored once and the other names are listed in ``__aliases__``
+("name=stored name"). The arrays are split over one file per group of layers so that every file
+stays below 1 MB. Arrays are NHWC float32; weights keep Caffe's [F][C][ky][kx] order."""
 import os
 import sys
 import tarfile
@@ -10,8 +14,24 @@ import tarfile
 import numpy
 
 SRC = "/root/reference/tests/functional/data/cifar_export.tar.xz"
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "data",
-                   "caffe_cifar_iter%d.npz")
+OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden",
+                   "caffe_replay")
+GROUPS = {"a": ("conv1",), "b": ("pool1", "relu1", "norm1"), "c": ("conv2", "pool2", "relu2", "norm2"),
+          "d": ("conv3", "pool3", "relu3", "ip1", "loss")}
+
+
+def used_keys():
+    keys = []
+    for g in GROUPS.values():
+        for n in g:
+            if n in ("ip1", "loss"):
+                continue
+            keys += [n + "/forward/bottom_0", n + "/forward/top_0", n + "/backward/top_err_0",
+                     n + "/backward/bottom_err_0"]
+            if n.startswith("conv"):
+                keys += [n + "/forward/blob_0", n + "/forward/blob_1"]
+    return keys + ["ip1/forward/bottom_0", "ip1/forward/blob_0", "ip1/forward/blob_1",
+                   "loss/forward/top_0", "ip1/backward/top_err_0", "ip1/backward/bottom_err_0"]
 
 
 def parse(text):
@@ -60,10 +80,22 @@ def main(iteration=0):
                 else:
                     val = numpy.ascontiguousarray(arr.transpose(0, 2, 3, 1))   # NCHW -> NHWC
                 out["%s/%s/%s" % (layer, direction, name)] = val.astype(numpy.float32)
-    path = OUT % iteration
-    os.makedirs(os.path.dirname(path), exist_ok=True)
-    numpy.savez_compressed(path, **out)
-    print(path, os.path.getsize(path), sorted(out)[:6], len(out))
+    stored, aliases = {}, []
+    for k in used_keys():
+        a = out[k]
+        same = [k2 for k2, a2 in stored.items() if a2.shape == a.shape and numpy.array_equal(a, a2)]
+        if same:
+            aliases.append("%s=%s" % (k, same[0]))
+        else:
+            stored[k] = a
+    os.makedirs(OUT, exist_ok=True)
+    for g, layers in GROUPS.items():
+        part = {k: a for k, a in stored.items() if k.split("/")[0] in layers}
+        if g == "a":
+            part["__aliases__"] = numpy.array(aliases)
+        path = os.path.join(OUT, "iter%d_%s.npz" % (iteration, g))
+        numpy.savez_compressed(path, **part)
+        print(path, os.path.getsize(path), len(part))
 
 
 if __name__ == "__main__":

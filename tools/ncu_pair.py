@@ -1,4 +1,4 @@
-"""Workload for `ncu --set full`: one 8192^3 bf16 GEMM on the 2-CTA kernel, one AlexNet conv2
+"""Workload for `ncu --set full`: one 8192^3 bf16 GEMM on the persistent kernel, one AlexNet conv2
 fprop / wgrad on the same kernel with the TMA im2col operand (a few launches each)."""
 import os
 import sys

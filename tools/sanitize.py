@@ -1,7 +1,7 @@
 """Small workloads for ``compute-sanitizer --tool {memcheck,racecheck,synccheck}``: every
 hand-rolled synchronisation protocol of the repo on sizes a sanitizer run can finish -
-gemm_umma_k (mbarrier ring, TMA + LDGSTS producers, TMEM), gemm_pair_k (cluster barriers,
-cta_group::2 TMA / commit multicast, remote mbarrier arrive), multi_update_k (grid barrier;
+gemm_umma_k (mbarrier ring, TMA + LDGSTS producers, wgmma), gemm_pair_k (producer / MMA
+warpgroups, TMA-store epilogue), lstm kernels (barrier.cluster), multi_update_k (grid barrier;
 fake-peer flag protocol with 2 ranks sharing the GPU), fc_small, pooling / LRN / evaluator."""
 import os
 import sys

@@ -1,4 +1,4 @@
-"""``veles`` namespace of the B200-native framework.
+"""``veles`` namespace of the H100-native framework.
 
 The real code lives in :mod:`veles.znicz_b200`. For users of the reference,
 reference-style import paths keep working through lazy aliases installed by

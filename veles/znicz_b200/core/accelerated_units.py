@@ -1,10 +1,10 @@
-"""AcceleratedUnit: a unit with a numpy oracle path and one sm_100a path.
+"""AcceleratedUnit: a unit with a numpy oracle path and one sm_90a path.
 
 Fresh design for ``veles.accelerated_units`` (AcceleratedUnit, AcceleratedWorkflow,
 TrivialAcceleratedUnit). The reference selects numpy/ocl/cuda per unit at run time
 (/root/reference/all2all.py:52, /root/reference/conv.py:70); here ``initialize(device)``
 binds ``run`` to ``numpy_run`` or ``cuda_run`` once. There is no JIT: kernels are
-ahead-of-time compiled for sm_100a in ``veles.znicz_b200.kernels``.
+ahead-of-time compiled for sm_90a in ``veles.znicz_b200.kernels``.
 """
 from __future__ import annotations
 

@@ -2,7 +2,7 @@
 real unit (a loader) can run ahead of the main contour
 (``veles.avatar.Avatar``; /root/reference/standard_workflow.py:386-404).
 
-On B200 the overlap itself is done with a copy stream + double buffered device
+On H100 the overlap itself is done with a copy stream + double buffered device
 minibatches inside the loader; the Avatar keeps the graph-level API: it clones the
 exported attributes on every run so downstream units read a stable snapshot.
 """

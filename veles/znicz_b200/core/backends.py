@@ -1,4 +1,4 @@
-"""Devices: ``NumpyDevice`` (CPU oracle) and ``CUDADevice`` (one B200, sm_100a).
+"""Devices: ``NumpyDevice`` (CPU oracle) and ``CUDADevice`` (one H100, sm_90a).
 
 Fresh design for ``veles.backends``. There is exactly one accelerator backend:
 no OpenCL, no multi-vendor dispatch (SURVEY "five facts" #2). A CUDADevice owns a
@@ -44,7 +44,7 @@ class NumpyDevice(Device):
 
 
 class CUDADevice(Device):
-    """One B200. The sm_100a extension is loaded eagerly and a missing/unloadable
+    """One H100. The sm_90a extension is loaded eagerly and a missing/unloadable
     extension is a hard error (never a silent fallback to eager PyTorch)."""
     is_cuda = True
     backend_name = "cuda"

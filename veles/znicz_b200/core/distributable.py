@@ -3,7 +3,7 @@
 The reference's only parallelism is the 5-method master/slave contract
 (/root/reference/nn_units.py:118,178-211,644-694). It is kept as API (tests drive
 it in-process, and the multi-process CPU path can use it over gloo), while the
-B200 data-parallel path is synchronous all-reduce fused with the update kernel
+H100 data-parallel path is synchronous all-reduce fused with the update kernel
 (``veles.znicz_b200.parallel``).
 """
 

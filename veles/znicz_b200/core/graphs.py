@@ -1,7 +1,7 @@
 """CUDA-graph capture of a chain of accelerated units.
 
 The reference drives >100 tiny kernel launches per minibatch from python
-(SURVEY §3.3). On B200 the python unit graph still decides *what* runs each
+(SURVEY §3.3). On H100 the python unit graph still decides *what* runs each
 minibatch, but a chain of units (forwards+evaluator, or all GD units) is captured
 once per gate configuration into a CUDA graph and replayed:
 

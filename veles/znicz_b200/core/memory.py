@@ -3,14 +3,14 @@
 Fresh design for ``veles.memory.Array`` (SURVEY §8 "Array protocol"; usages
 /root/reference/nn_units.py:145,157-160,196-205,375, /root/reference/all2all.py:262,
 /root/reference/evaluator.py:506-513). ``.mem`` is the numpy view, ``.devmem`` is a
-``torch.Tensor`` living in B200 HBM. The map_read/map_write/map_invalidate/unmap
+``torch.Tensor`` living in H100 HBM. The map_read/map_write/map_invalidate/unmap
 API is kept as a thin coherence state machine:
 
     MAPPED_READ   host valid, device valid
     MAPPED_WRITE  host valid, device stale   (unmap() uploads)
     UNMAPPED      device owns the data       (map_read() downloads)
 
-B200 departures: the device copy may use a narrower dtype than the host copy
+H100 departures: the device copy may use a narrower dtype than the host copy
 (``dev_dtype`` = bf16 activations while ``.mem`` stays float32), and all device
 buffers are ordinary torch allocations so CUDA graphs can capture kernels that
 read and write them.

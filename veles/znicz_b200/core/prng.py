@@ -2,7 +2,7 @@
 
 Used by the reference for weight filling (``rand.fill``, ``fill_normal_real``
 /root/reference/all2all.py:119-127), loader shuffling and dropout/stochastic-pooling
-seeds. Device-side randomness on B200 is counter-based (Philox-style hash of
+seeds. Device-side randomness on H100 is counter-based (Philox-style hash of
 (seed, step, element)) inside the kernels, so no per-element state arrays exist;
 the host generator only provides the seeds.
 """

@@ -13,7 +13,7 @@ the reference consumes (SURVEY §8 "Unit protocol"; usages
   by ``init_unpickled()``
 
 Scheduling is a deterministic single-threaded FIFO walk owned by the Workflow
-(one CUDA stream is the real executor on the B200 path; python only decides
+(one CUDA stream is the real executor on the H100 path; python only decides
 *what* is enqueued), not the reference core's thread pool.
 """
 from __future__ import annotations

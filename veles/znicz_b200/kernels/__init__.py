@@ -1,4 +1,4 @@
-"""sm_100a kernels of znicz_b200 (hand-written CUDA, ahead-of-time compiled, in-tree)."""
+"""sm_90a kernels of znicz_b200 (hand-written CUDA, ahead-of-time compiled, in-tree)."""
 from __future__ import annotations
 
 import importlib.util
@@ -19,7 +19,7 @@ def load_extension(required=True):
         if required:
             raise RuntimeError(
                 "znicz_b200: %s is missing. Build it with "
-                "`python -m veles.znicz_b200.kernels.build` (nvcc cross-compiles sm_100a "
+                "`python -m veles.znicz_b200.kernels.build` (nvcc cross-compiles sm_90a "
                 "without a GPU)." % SO_PATH)
         return None
     import torch  # noqa: F401  (libtorch must be loaded first)

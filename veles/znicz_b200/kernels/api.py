@@ -1,4 +1,4 @@
-"""Glue between the unit classes and the sm_100a extension.
+"""Glue between the unit classes and the sm_90a extension.
 
 Every function takes a unit, pulls the device tensors out of its Arrays
 (``.dev`` = read, ``.dev_out`` = about to be overwritten) and launches kernels on the
@@ -6,9 +6,9 @@ current CUDA stream. Nothing here synchronises with the host or allocates per ca
 (temporaries are cached on the unit), so every function is CUDA-graph capturable.
 
 Engine selection is by *shape legality*, not by backend: bf16 activations + TMA-legal
-leading dimensions go through the tcgen05 kernels (``gemm_umma.cu``); everything else
+leading dimensions go through the wgmma kernels (``gemm_umma.cu``); everything else
 (fp32 compute type, leading dims that are not multiples of 8 elements, transposed weight
-storage) runs the exact-fp32 SIMT implicit-GEMM kernels. A tcgen05 launcher that refuses
+storage) runs the exact-fp32 SIMT implicit-GEMM kernels. A wgmma launcher that refuses
 a shape raises — there is no silent fallback to PyTorch.
 """
 from __future__ import annotations
@@ -22,6 +22,17 @@ from ..core.config import root
 from ..ops.nn_units import ACT_LINEAR
 
 _MAX_SPLITS = 64
+_SMS = {}
+
+
+def _num_sms():
+    """Streaming multiprocessors of the current CUDA device (split-K sizing aims at two CTAs each)."""
+    d = torch.cuda.current_device()
+    if d not in _SMS:
+        _SMS[d] = torch.cuda.get_device_properties(d).multi_processor_count
+    return _SMS[d]
+
+
 counters = {"launches": 0}
 
 
@@ -31,7 +42,7 @@ from . import fp32x  # noqa: E402
 def _ext(unit):
     ext = unit.ext_
     if ext is None:
-        raise RuntimeError("%s: the sm_100a extension is not loaded" % unit)
+        raise RuntimeError("%s: the sm_90a extension is not loaded" % unit)
     return ext
 
 
@@ -180,7 +191,7 @@ def fc_forward(unit, softmax=False):
         r = ext.gemm(x, n_in, False, w, w.shape[1], True, out, n_out, False,
                      batch, n_out, n_in, bias, act, 1.0, 0.0, 1, 0, 1)
         if r != 0:
-            raise RuntimeError("%s: tcgen05 FC forward refused the shape (code %d)" % (unit, r))
+            raise RuntimeError("%s: wgmma FC forward refused the shape (code %d)" % (unit, r))
     elif fp32x.enabled(unit) and fp32x.fc_forward(unit, ext, x, out, bias, act, batch, n_in,
                                                   n_out):
         pass          # fp32 operands as bf16 hi/lo parts on the tensor cores (kernels/fp32x.py)
@@ -215,7 +226,7 @@ def _warn_once(unit, what, code):
     key = (id(unit), what)
     if key not in _WARNED:
         _WARNED.add(key)
-        unit.warning("tcgen05 %s kernel declined this shape (code %d): using the SIMT kernel",
+        unit.warning("wgmma %s kernel declined this shape (code %d): using the SIMT kernel",
                      what, code)
 
 
@@ -232,7 +243,7 @@ def _fc_small_ok(unit, n_out):
 # dgrad and wgrad of a layer both only *read* err_output, and nothing consumes the weight gradient
 # before the optimizer step: the wgrad kernels run on the device's side stream (a parallel branch
 # of the captured graph) while the main stream carries the err_input chain down the network. The
-# small-grid kernels of small nets (50-200 CTAs) then share the 148 SMs instead of queueing.
+# small-grid kernels of small nets (50-200 CTAs) then share the SMs instead of queueing.
 def _fork_side(unit):
     dev = unit.device
     if not root.common.engine.get("overlap_wgrad", True) or getattr(dev, "side_stream", None) is None:
@@ -404,7 +415,7 @@ def fc_backward(unit):
                          batch, n_in, n_out, None, 0, float(unit.err_input_alpha),
                          float(unit.err_input_beta), 1, 0, 1)
             if r != 0:
-                raise RuntimeError("%s: tcgen05 FC dgrad refused (code %d)" % (unit, r))
+                raise RuntimeError("%s: wgmma FC dgrad refused (code %d)" % (unit, r))
         else:
             _path(unit, "fc_dgrad:simt(lp_ok=%s,err=%s,x=%s,lp=%s)" % (
                 lp_ok, err.dtype, x.dtype,
@@ -426,7 +437,7 @@ def fc_backward(unit):
         r = -1
         if lp_ok and n_out % 8 == 0 and n_in % 8 == 0 and n_out >= 256 and n_in >= 256 \
                 and batch >= 64:
-            # large layers: err^T . x on the 2-CTA persistent kernel (both operands MN-major,
+            # large layers: err^T . x on the persistent kernel (both operands MN-major,
             # TMA-store epilogue straight into the [neurons][in] gradient layout)
             r = int(ext.fc_wgrad_pair(err.view(batch, n_out), x.view(batch, n_in),
                                        gbuf.view(n_out, n_in)))
@@ -442,7 +453,7 @@ def fc_backward(unit):
             r = ext.gemm(x, n_in, True, err, n_out, False, gbuf, n_in, True,
                          n_in, n_out, batch, None, 0, 1.0, 0.0, 1, 0, 1)
             if r != 0:
-                raise RuntimeError("%s: tcgen05 FC wgrad refused (code %d)" % (unit, r))
+                raise RuntimeError("%s: wgmma FC wgrad refused (code %d)" % (unit, r))
         else:
             _path(unit, "fc_wgrad:simt")
             ext.gemm(err, n_out, True, x, n_in, False, gbuf,
@@ -536,7 +547,7 @@ def conv_forward(unit):
             ext.conv_fprop(unit.input.dev, w, w.shape[1], bool(unit.weights_transposed), bias,
                            out, _conv_geom(unit), eff_act(unit), 0)
         elif r != 0:
-            raise RuntimeError("%s: tcgen05 conv fprop refused (code %d)" % (unit, r))
+            raise RuntimeError("%s: wgmma conv fprop refused (code %d)" % (unit, r))
     elif fp32x.enabled(unit) and fp32x.conv_forward(unit, ext, x, out, bias, g, eff_act(unit)):
         pass          # (kernels/fp32x.py counts its split launches itself)
     else:
@@ -562,7 +573,7 @@ def conv_backward(unit):
     act = eff_act(unit)
     if unit.__dict__.get("deriv_upstream_"):
         act = ACT_LINEAR       # the consumer's backward kernel already applied f'(y) (fusion.py)
-    # bias gradient: with nothing to multiply into err_output, the tcgen05 wgrad kernel delivers the
+    # bias gradient: with nothing to multiply into err_output, the wgmma wgrad kernel delivers the
     # column sums as an extra product row (no separate pass over err_output at all)
     bias_row = bool(need_b and act == ACT_LINEAR and lp_ok)
     parts = slices = None
@@ -614,7 +625,7 @@ def conv_backward(unit):
                 fold = False
             folded = fold and r == 0
             if r not in (0, -3, -4):
-                raise RuntimeError("%s: tcgen05 conv dgrad refused (code %d)" % (unit, r))
+                raise RuntimeError("%s: wgmma conv dgrad refused (code %d)" % (unit, r))
             if r != 0:
                 _warn_once(unit, "dgrad", r)
         if r != 0:
@@ -674,7 +685,7 @@ def conv_backward(unit):
         splits = int(ext.pick_splits(kw, f_rows, pixels, _MAX_SPLITS))
     else:
         tiles = ((f + 63) // 64) * ((kw + 63) // 64)
-        splits = max(1, min(_MAX_SPLITS, (2 * 148) // tiles, (pixels + 255) // 256))
+        splits = max(1, min(_MAX_SPLITS, (2 * _num_sms()) // tiles, (pixels + 255) // 256))
     gbuf = _grad_buffer(unit, "wgrad", (splits, f_rows, kw)) if s2d is None else \
         _tmp(unit, "wgrad_s2d", (splits, f_rows, kw), torch.float32)
     brow = None
@@ -684,7 +695,7 @@ def conv_backward(unit):
         if use_umma:
             r = ext.conv_wgrad(err_mm, x, gbuf, splits, g, False, 1, brow)
             if r not in (0, 1):
-                raise RuntimeError("%s: tcgen05 conv wgrad refused (code %d)" % (unit, r))
+                raise RuntimeError("%s: wgmma conv wgrad refused (code %d)" % (unit, r))
             if r == 0:
                 brow = None
             if s2d is not None:
@@ -905,7 +916,7 @@ def _rhits(unit, like):
 def _deconv_owner(unit):
     """The Conv unit that owns the (tied) weights of a Deconv / GDDeconv: its bf16 operand
     shadows (``weights_lp_`` [F][ld] and ``weights_lp_t_`` [tap][F_pad][C_pad]) are exactly what
-    the tcgen05 kernels need with the roles swapped (deconv forward = conv dgrad, GDDeconv
+    the wgmma kernels need with the roles swapped (deconv forward = conv dgrad, GDDeconv
     err_input = conv fprop, GDDeconv wgrad = conv wgrad with image and error exchanged)."""
     o = unit.__dict__.get("shadow_owner_", False)
     if o is not False:
@@ -948,7 +959,7 @@ def deconv_forward(unit):
         wd = o.weights_lp_t_
         r = int(ext.conv_dgrad(x, wd, wd.shape[1], False, out, g, alpha, 0.0, 1, None, 0))
         if r not in (0, -3, -4):
-            raise RuntimeError("%s: tcgen05 deconv (dgrad kernel) refused (code %d)" % (unit, r))
+            raise RuntimeError("%s: wgmma deconv (dgrad kernel) refused (code %d)" % (unit, r))
         if r != 0:
             _warn_once(unit, "deconv", r)
     if r != 0:
@@ -994,7 +1005,7 @@ def deconv_backward(unit):
             w = o.weights_lp_
             r = int(ext.conv_fprop(img, w, w.shape[1], False, None, dst, g_lp, 0, 1))
             if r not in (0, -3, -4):
-                raise RuntimeError("%s: tcgen05 GDDeconv err_input refused (code %d)" % (unit, r))
+                raise RuntimeError("%s: wgmma GDDeconv err_input refused (code %d)" % (unit, r))
             if r != 0:
                 _warn_once(unit, "gd_deconv err_input", r)
         if r != 0:
@@ -1017,12 +1028,12 @@ def deconv_backward(unit):
         gbuf = _grad_buffer(unit, "wgrad", (splits, f, kw_lp))
         r = int(ext.conv_wgrad(xin, img, gbuf, splits, g_lp, False, 1, None))
         if r not in (0, 1):
-            raise RuntimeError("%s: tcgen05 GDDeconv wgrad refused (code %d)" % (unit, r))
+            raise RuntimeError("%s: wgmma GDDeconv wgrad refused (code %d)" % (unit, r))
         _launch()
         _update(unit, False, gbuf, splits, f * kw_lp, f, kw, g_cpad=cp)
         return
     tiles = ((f + 63) // 64) * ((kw + 63) // 64)
-    splits = max(1, min(_MAX_SPLITS, (2 * 148) // tiles, (pixels + 255) // 256))
+    splits = max(1, min(_MAX_SPLITS, (2 * _num_sms()) // tiles, (pixels + 255) // 256))
     gbuf = _grad_buffer(unit, "wgrad", (splits, f, kw))
     ext.conv_wgrad(unit.input.dev, err, gbuf, splits, g, bool(unit.weights_transposed), 0, None)
     _launch()
@@ -1033,12 +1044,12 @@ def deconv_backward(unit):
 # LSTM over a sequence (ops/lstm_seq.py)
 # ------------------------------------------------------------------------------------------
 def _lstm_gemm_nt(ext, unit, a, w_lp, w_f32, out, m, n, k, bias, beta):
-    """out[m, n] = a[m, k] . W[n, k]^T (+ bias) (+ beta * out); tcgen05 when a is bf16."""
+    """out[m, n] = a[m, k] . W[n, k]^T (+ bias) (+ beta * out); wgmma when a is bf16."""
     if w_lp is not None and _is_bf16(a) and k % 8 == 0:
         r = ext.gemm(a, k, False, w_lp, w_lp.shape[1], True, out, n, False, m, n, k, bias,
                      ACT_LINEAR, 1.0, beta, 1, 0, 1)
         if r != 0:
-            raise RuntimeError("%s: tcgen05 LSTM GEMM refused (code %d)" % (unit, r))
+            raise RuntimeError("%s: wgmma LSTM GEMM refused (code %d)" % (unit, r))
     else:
         ext.gemm(a, k, False, w_f32, k, True, out, n, False, m, n, k, bias, ACT_LINEAR, 1.0,
                  beta, 1, 0, 0)
@@ -1078,7 +1089,7 @@ def lstm_seq_forward(unit):
     state = None
     if w_lp is not None and _lstm_persist_enabled():
         # the whole time loop in ONE cluster launch: W resident in shared memory, gates GEMM on
-        # tcgen05, cell math in the epilogue, h exchanged through distributed shared memory
+        # wgmma, cell math in the epilogue, h exchanged through distributed shared memory
         # (csrc/lstm_persist.cu)
         nstate = int(ext.lstm_state_floats(t, b, i, h))
         if nstate:
@@ -1150,7 +1161,7 @@ def lstm_seq_backward(unit):
             r = ext.gemm(dz.view(t * b, h4), h4, False, w_lp, w_lp.shape[1], False, dx, i, False,
                          t * b, i, h4, None, 0, 1.0, 0.0, 1, 0, 1)
             if r != 0:
-                raise RuntimeError("%s: tcgen05 LSTM dx refused (code %d)" % (unit, r))
+                raise RuntimeError("%s: wgmma LSTM dx refused (code %d)" % (unit, r))
             ext.swap01_2d(dx, i, 0, ei, i, 0, t, b, i)
             _launch(2)
     for s in range(t - 1 if persist != 0 else -1, -1, -1):
@@ -1168,7 +1179,7 @@ def lstm_seq_backward(unit):
                 r = ext.gemm(dz[s], h4, False, w_lp, w_lp.shape[1], False, dxh, i + h, False,
                              b, i + h, h4, None, 0, 1.0, 0.0, 1, 0, 1)
                 if r != 0:
-                    raise RuntimeError("%s: tcgen05 LSTM dgrad refused (code %d)" % (unit, r))
+                    raise RuntimeError("%s: wgmma LSTM dgrad refused (code %d)" % (unit, r))
             else:
                 ext.gemm(dz[s], h4, False, w, i + h, False, dxh, i + h, False, b, i + h, h4,
                          None, 0, 1.0, 0.0, 1, 0, 0)
@@ -1190,7 +1201,7 @@ def lstm_seq_backward(unit):
         r = ext.gemm(dz2, h4, True, xh2, i + h, False, gbuf, i + h, False, h4, i + h, rows,
                      None, 0, 1.0, 0.0, 1, 0, 1)
         if r != 0:
-            raise RuntimeError("%s: tcgen05 LSTM wgrad refused (code %d)" % (unit, r))
+            raise RuntimeError("%s: wgmma LSTM wgrad refused (code %d)" % (unit, r))
     else:
         ext.gemm(dz2, h4, True, xh2, i + h, False, gbuf, i + h, False, h4, i + h, rows, None, 0,
                  1.0, 0.0, 1, 0, 0)

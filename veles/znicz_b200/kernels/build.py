@@ -1,7 +1,7 @@
-"""Ahead-of-time build of the sm_100a extension, in-tree.
+"""Ahead-of-time build of the sm_90a extension, in-tree.
 
 ``python -m veles.znicz_b200.kernels.build`` compiles every ``csrc/*.cu`` with
-``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` (cross-compiles without a GPU),
+``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` (cross-compiles without a GPU),
 ``csrc/ext.cpp`` against the torch headers, and links ``_znicz_b200_C.so`` next to this
 file so the binary travels with the source tree (no JIT cache, no site-packages install).
 """
@@ -20,7 +20,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 SO_NAME = "_znicz_b200_C.so"
 SO_PATH = os.path.join(HERE, SO_NAME)
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr"]
 
@@ -43,7 +43,8 @@ def _sources():
 
 
 def source_digest():
-    h = hashlib.sha1()
+    # the flags are part of the digest: an extension built for another architecture is stale
+    h = hashlib.sha1(" ".join(ARCH_FLAGS + NVCC_FLAGS).encode())
     for f in sorted(os.listdir(CSRC)):
         if f.endswith((".cu", ".cuh", ".cpp", ".h")):
             with open(os.path.join(CSRC, f), "rb") as fin:

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels of znicz_b200.
+// Shared device helpers for the sm_90a kernels of znicz_b200.
 // No torch headers here: .cu files compile in seconds; ext.cpp does the binding.
 #pragma once
 #include <cuda_runtime.h>
@@ -14,7 +14,7 @@ namespace zn {
 // Every kernel of the step is launched with the programmatic-stream-serialization attribute
 // (also inside captured CUDA graphs, where it becomes a programmatic edge): kernel N+1's CTAs are
 // scheduled as soon as all CTAs of kernel N have started, run their prologue (index math, smem
-// carve-up, barrier init, TMEM allocation) and block in pdl_wait() until kernel N has completed
+// carve-up, barrier init) and block in pdl_wait() until kernel N has completed
 // and flushed. The ~25 launches of a training step otherwise pay one full drain + launch latency
 // each. ZNICZ_PDL=0 switches the attribute off (plain stream order).
 #ifndef ZN_PDL_EARLY_TRIGGER
@@ -32,6 +32,18 @@ inline bool pdl_enabled() {
   static int on = -1;
   if (on < 0) { const char* e = getenv("ZNICZ_PDL"); on = (e && atoi(e) == 0) ? 0 : 1; }
   return on != 0;
+}
+
+// streaming multiprocessors of the current device (132 on an H100 SXM), queried once
+inline int num_sms() {
+  static int n = 0;
+  if (!n) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (n < 1) n = 132;
+  }
+  return n;
 }
 
 template <typename... KArgs, typename... Args>
@@ -113,7 +125,7 @@ __device__ __forceinline__ float act_fwd(int act, float s, float factor = 1.f, i
 }
 // The five layer activations that can sit in a GEMM/conv epilogue. Small code on purpose: the
 // generic act_fwd() drags sinf/cosf/logf slow paths into every unrolled epilogue element and
-// made the tcgen05 kernels ~45k SASS instructions (instruction-fetch bound).
+// made the wgmma kernels ~45k SASS instructions (instruction-fetch bound).
 __device__ __forceinline__ float act_fwd5(int act, float s) {          // accurate (fp32 paths)
   if (act == ACT_LINEAR) return s;
   if (act == ACT_STRICT_RELU) return fmaxf(s, 0.f);

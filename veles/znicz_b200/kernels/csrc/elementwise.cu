@@ -242,7 +242,7 @@ __global__ void gather_minibatch_k(const TS* __restrict__ src, const int* __rest
   const int* idx = hdr + 4;
   const int total = max_rows * row8;
   if (dst_pad) {
-    // second copy with the channels padded C -> CP (= 8): the first conv layer's tcgen05 gather
+    // second copy with the channels padded C -> CP (= 8): the first conv layer's wgmma gather
     // then moves whole 16-byte pixels (replaces a separate pad_channels launch)
     const int pixels = row8 * 8 / C;
     const int ptotal = max_rows * pixels;
@@ -386,9 +386,9 @@ void launch_gather_rows(const void* src, bool src_bf16, const int* idx, void* ds
   else launch_k(gather_rows_k<__nv_bfloat16, float>, g, 256, 0, st, (const __nv_bfloat16*)src, idx, (float*)dst, count, max_rows, row);
 }
 // Host -> device "pull": the SMs read a pinned (mapped) host buffer directly over PCIe and write
-// device memory. Used instead of cudaMemcpyAsync for the per-step loader uploads: on this platform
-// every switch between the copy engine and compute work in one stream costs ~100 us (measured,
-// profiles/host_vs_device_r1.md), a kernel reading host memory costs one PCIe round trip.
+// device memory. Used instead of cudaMemcpyAsync for the per-step loader uploads: a switch between
+// the copy engine and compute work in one stream is costly, a kernel reading host memory costs one
+// PCIe round trip.
 // ld.global.cv: never serve a slot the host has rewritten since from a cached line.
 __global__ void pull_from_host_k(const uint4* __restrict__ src, uint4* __restrict__ dst, long long n16,
                                  const unsigned char* __restrict__ src_b, unsigned char* __restrict__ dst_b,
@@ -403,7 +403,7 @@ void launch_pull_from_host(const void* src_dev_alias, void* dst, long long nbyte
   const long long n16 = nbytes / 16;
   const int tail = (int)(nbytes - n16 * 16);
   long long blocks = (n16 + 255) / 256;
-  if (blocks > 592) blocks = 592;
+  if (blocks > 4 * num_sms()) blocks = 4 * num_sms();
   if (blocks < 1) blocks = 1;
   launch_k(pull_from_host_k, (int)blocks, 256, 0, st, (const uint4*)src_dev_alias, (uint4*)dst, n16,
            (const unsigned char*)src_dev_alias + n16 * 16, (unsigned char*)dst + n16 * 16, tail);

@@ -1,4 +1,4 @@
-// Python bindings of the znicz_b200 sm_100a kernels (the only file that sees torch headers).
+// Python bindings of the znicz_b200 sm_90a kernels (the only file that sees torch headers).
 #include <torch/extension.h>
 #include <c10/cuda/CUDAStream.h>
 #include <cuda_runtime.h>
@@ -326,7 +326,7 @@ void device_copy(Tensor src, Tensor dst) {
   zn::launch_pull_from_host(src.data_ptr(), dst.data_ptr(), nbytes, cur());
   kcheck();
 }
-// ---- fp8: per-tensor e4m3 quantisation + tcgen05 kind::f8f6f4 GEMM (first slice of the fp8 path)
+// ---- fp8: per-tensor e4m3 quantisation + wgmma e4m3 GEMM (first slice of the fp8 path)
 void fp8_absmax(Tensor x, Tensor amax) {
   chk(x, "x");
   TORCH_CHECK(amax.is_cuda() && amax.scalar_type() == torch::kFloat32 && amax.numel() >= 1);
@@ -689,7 +689,7 @@ int64_t gemm(Tensor a, int64_t lda, bool transa, Tensor b, int64_t ldb, bool tra
              int64_t act, double alpha, double beta, int64_t splits, int64_t split_stride, int64_t engine) {
   chk(a, "a"); chk(b, "b"); chk(out, "out");
   if (engine == 1) {
-    TORCH_CHECK(is_bf16(a) && is_bf16(b), "tcgen05 path needs bf16 operands");
+    TORCH_CHECK(is_bf16(a) && is_bf16(b), "wgmma path needs bf16 operands");
     int r = zn::launch_gemm_umma(a.data_ptr(), lda, transa ? 1 : 0, b.data_ptr(), ldb, transb ? 0 : 1,
                                  out.data_ptr(), is_bf16(out) ? 1 : 0, ldo, out_trans ? 1 : 0, (int)M,
                                  (int)N, (int)K, fptr_or_null(bias), (int)act, (float)alpha, (float)beta,
@@ -704,7 +704,7 @@ int64_t gemm(Tensor a, int64_t lda, bool transa, Tensor b, int64_t ldb, bool tra
   kcheck();
   return 0;
 }
-// 2-CTA persistent tcgen05 GEMM (gemm_pair.cu): out[M][N] = act(alpha * a[M][K] . b[N][K]^T + bias)
+// persistent warp-specialised wgmma GEMM (gemm_pair.cu): out[M][N] = act(alpha * a[M][K] . b[N][K]^T + bias)
 int64_t gemm_pair(Tensor a, Tensor b, Tensor out, c10::optional<Tensor> bias, int64_t act, double alpha) {
   chk(a, "a"); chk(b, "b"); chk(out, "out");
   TORCH_CHECK(is_bf16(a) && is_bf16(b) && a.dim() == 2 && b.dim() == 2 && out.dim() == 2);
@@ -716,7 +716,7 @@ int64_t gemm_pair(Tensor a, Tensor b, Tensor out, c10::optional<Tensor> bias, in
   if (r == 0) kcheck();
   return r;
 }
-// FC weight gradient on the 2-CTA kernel: out[n_out][n_in] fp32 = err[batch][n_out]^T . x[batch][n_in]
+// FC weight gradient on the persistent kernel: out[n_out][n_in] fp32 = err[batch][n_out]^T . x[batch][n_in]
 int64_t fc_wgrad_pair(Tensor err, Tensor x, Tensor out) {
   chk(err, "err"); chk(x, "x"); chk(out, "out");
   TORCH_CHECK(is_bf16(err) && is_bf16(x) && out.scalar_type() == torch::kFloat32);
@@ -1031,7 +1031,7 @@ void host_prefetch_wait(int64_t ticket) { znhost::HostPrefetcher::get().wait((ui
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("som_winners", &som_winners); m.def("som_update", &som_update);
-  m.doc() = "znicz_b200 sm_100a kernels";
+  m.doc() = "znicz_b200 sm_90a kernels";
   m.def("act_forward", &act_forward); m.def("act_backward", &act_backward);
   m.def("colsum_slices", &colsum_slices); m.def("err_act_colsum", &err_act_colsum);
   m.def("dropout_forward", &dropout_forward); m.def("binary_op", &binary_op);

@@ -1,7 +1,7 @@
 // Fully connected layers with a handful of outputs (n_out <= 16: the 10-class softmax head of the
 // CIFAR/MNIST nets, Wine's 3 classes, the 7-segment targets of Mnist7 ...).
 //
-// A 128x16 tcgen05 tile wastes > 90 % of the tensor-core tile for N = 10 and the generic SIMT GEMM
+// A 128x16 wgmma tile wastes > 90 % of the tensor-core tile for N = 10 and the generic SIMT GEMM
 // is latency bound at 16 CTAs, so these shapes get two purpose-built kernels:
 //
 //   fc_small_forward_k   one CTA per batch row: dot products against all outputs, bias, activation

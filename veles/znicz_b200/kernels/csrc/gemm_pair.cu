@@ -1,26 +1,23 @@
-// Dense GEMM for large shapes, Blackwell 2-CTA form (sm_100a):
+// Dense GEMM for large shapes, persistent warp-specialised form (sm_90a):
 //
-//   D[M, N] = act(alpha * sum_k A[m, k] * B[n, k] + bias[n])        A, B bf16 K-major, D bf16 / fp32
+//   D[M, N] = act(alpha * sum_k A[m, k] * B[n, k] + bias[n])        A, B bf16, D bf16 / fp32
 //
-// * a CLUSTER OF TWO CTAs (one TPC) owns a 256 x BN tile: `tcgen05.mma.cta_group::2` with
-//   UMMA_M = 256, each CTA stages its own 128 rows of A and only HALF of the B tile (BN / 2 rows)
-//   - the tensor core reads both halves across the pair, so B's shared-memory and L2 traffic per
-//   SM is halved against two independent 128-row tiles;
-// * TMA loads `.cta_group::2`: both CTAs' copies complete on the LEADER's mbarrier (one wait for
-//   the MMA issuer), a deep ring (6 x 32 KB stages at BN = 256);
-// * PERSISTENT: 74 clusters loop over the tiles (grouped raster: 8 M-tiles x all N-tiles per
-//   group, so a wave re-reads A and B from L2), the accumulator is DOUBLE BUFFERED in TMEM
-//   (2 x BN fp32 columns = all 512 columns at BN = 256): the epilogue of tile t (TMEM -> registers
-//   -> bias / activation -> swizzled smem -> TMA store) overlaps the MMAs of tile t + 1;
-// * warp roles: 0 = TMA producer, 1 = MMA issuer (leader CTA only), 2 = TMEM allocation,
-//   4..7 = epilogue (lane l of warp 4 + w owns accumulator row 32 w + l).
+// * one CTA per SM loops over 128 x BN output tiles (grouped raster: 8 M-tiles x all N-tiles per
+//   group, so a wave re-reads A and B from L2);
+// * warpgroup 0 is the producer (one thread issues the TMA loads of a deep ring: 4 x 48 KB stages
+//   at BN = 256, 6 x 32 KB at BN = 128) and hands its registers to the two MMA warpgroups;
+// * warpgroups 1 and 2 each own 64 rows of the tile: wgmma m64 x BN x k16 with the fp32
+//   accumulators in registers, then the epilogue (bias / activation / f' -> swizzled smem -> TMA
+//   store, two staging buffers so the store of one chunk overlaps the next);
+// * the ring runs ahead across tiles: the loads of tile t + 1 are in flight during the epilogue
+//   of tile t.
 //
-// Used for the 8192^3-class GEMMs and the large fully-connected layers (perf shape of the
-// reference: /root/reference/tests/unit/test_all2all.py:98-127); skinny / small shapes stay on
-// gemm_umma.cu. The single-CTA kernel reached 46 % of cuBLAS on 8192^3 (profiles/roofline_r1.md).
+// Used for the large fully-connected layers and convolutions; skinny / small shapes stay on
+// gemm_umma.cu.
 #include "common.cuh"
 #include "umma.cuh"
 #include <stdlib.h>
+#include <utility>
 
 namespace zn {
 
@@ -28,11 +25,11 @@ using namespace umma;
 
 namespace pr {
 
-constexpr int BM = 128;                 // rows per CTA; the pair's UMMA_M is 256
+constexpr int BM = 128;                 // rows per tile (two 64-row MMA warpgroups)
 constexpr int BK = 64;                  // bf16 elements = 128 bytes = one SW128 row
 constexpr int A_BYTES = BM * 128;
 constexpr int EPI_BUF = 128 * 128;      // 128 rows x 128 bytes per staging buffer
-constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;   // clears the CTA-rank bit: "same variable in CTA 0"
+constexpr int THREADS = 384;
 
 // A operand: dense [M][K] tile, or the implicit-GEMM operand of a convolution fetched by TMA in
 // im2col mode (one [128 pixels x 64 channels] box per k-block): fprop = im2col(x), dgrad
@@ -54,75 +51,6 @@ struct Params {
   const __nv_bfloat16* dmul; int dact; long long ldo;   // dgrad: out *= f'(dmul[row][col])
 };
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem, both CTAs] (+)= A[smem of both CTAs: 2 x 128 rows] * B[smem of both CTAs: 2 x BN/2 rows]
-__device__ __forceinline__ void mma_f16_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all MMAs issued so far -> one arrival on `bar` in EVERY CTA of the mask
-__device__ __forceinline__ void mma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-          "r"(smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-// tile -> this CTA's shared memory, completion bytes -> the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* map, uint64_t* bar,
-                                                int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1)
-      : "memory");
-}
-// im2col-mode load (see umma.cuh::tma_load_im2col_4d), 2-CTA form: bytes complete on CTA 0's barrier
-__device__ __forceinline__ void tma_load_im2col_2sm(void* smem_dst, const CUtensorMap* map, uint64_t* bar,
-                                                    int c, int w, int h, int n, uint16_t off_w,
-                                                    uint16_t off_h) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};" ::"r"(smem_u32(smem_dst)),
-      "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 __device__ __forceinline__ void tma_store_wait_read(int keep) {
   if (keep == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
   else asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
@@ -139,94 +67,81 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   tm = m0 + (r - tn * gm);
 }
 
+template <typename F, int... I>
+__device__ __forceinline__ void static_for(std::integer_sequence<int, I...>, F&& f) {
+  (f(std::integral_constant<int, I>{}), ...);
+}
+
+template <int BN>
+__host__ __device__ constexpr int pair_stages() { return BN == 256 ? 4 : 6; }
+
 template <int BN, bool OUT_F32, int AMODE = AM_DENSE, int BMODE = BM_K>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_c, const Params p) {
-  constexpr int B_BYTES = (BN / 2) * 128;
+  constexpr int B_BYTES = BN * 128;
   constexpr int STAGE = A_BYTES + B_BYTES;
-  constexpr int NST = (BN == 256) ? 6 : 8;
+  constexpr int NST = pair_stages<BN>();
   constexpr int EPI_COLS = OUT_F32 ? 32 : 64;          // 128-byte staging rows
   constexpr int NCHUNK = BN / EPI_COLS;
+  constexpr int ESZ = OUT_F32 ? 4 : 2;
   constexpr bool A_MN = (AMODE == AM_DENSE_MN);
   constexpr bool B_MN = (BMODE != BM_K);
-  constexpr uint32_t IDESC = make_idesc_bf16(2 * BM, BN, A_MN ? 1 : 0, B_MN ? 1 : 0);
-  constexpr uint32_t TMEM_COLS = 2 * BN;               // double-buffered accumulator (256 or 512)
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[NST];
   __shared__ __align__(8) uint64_t empty_bar[NST];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
 
   uint8_t* tiles = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* epi = tiles + (size_t)NST * STAGE;          // 2 x EPI_BUF, 1024-byte aligned
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cid = blockIdx.x >> 1, nclusters = gridDim.x >> 1;
+  const int wg = warp >> 2;
   const int splits = p.splits > 1 ? p.splits : 1;
   const int num_tiles = p.tiles_m * p.tiles_n * splits;      // work items (tile, k-split)
   const int total_kb = (p.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 1u); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full_bar[a], 1u); mbar_init(&tmem_empty_bar[a], 8u); }
+    for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 2u); }
     fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a); tma_prefetch_desc(&tmap_b); tma_prefetch_desc(&tmap_c);
   }
-  if (warp == 2) { tmem_alloc2(&tmem_base_smem, TMEM_COLS); tmem_relinquish2(); }
-  tc_fence_before();
-  cluster_sync_all();            // barriers of both CTAs initialised before any remote signal
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
+  __syncthreads();
 
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (lane == 0) {
+  if (wg == 0) {
+    // ===================== producer warpgroup =====================
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       uint32_t it = 0;
-      for (int t = cid; t < num_tiles; t += nclusters) {
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         int tm, tn;
         tile_coords(t / splits, p.tiles_m, p.tiles_n, tm, tn);
         const int split = t % splits;
         const int kb0 = split * p.kb_per_split;
         const int kb1 = splits > 1 ? min(total_kb, kb0 + p.kb_per_split) : total_kb;
-        const int m0 = tm * 2 * BM + (int)rank * BM;
-        const int n0 = tn * BN + (int)rank * (BN / 2);
+        const int m0 = tm * BM, n0 = tn * BN;
         for (int kb = kb0; kb < kb1; ++kb, ++it) {
           const int s = it % NST; const uint32_t ph = (it / NST) & 1;
           mbar_wait(&empty_bar[s], ph ^ 1);
           uint8_t* sa = tiles + (size_t)s * STAGE;
-          // the leader's barrier expects the bytes of BOTH CTAs; the peer's copies may complete
-          // before this expect_tx is posted (the tx-count just goes negative for a moment)
-          uint32_t tx = 2u * STAGE;
-          int nblk = BN / 128;                 // 64-wide B blocks this CTA loads (im2col B only)
+          uint32_t tx = STAGE;
+          int nblk = BN / 64;                  // 64-wide B blocks (im2col B only)
           if (BMODE == BM_IM2COL_MN) {
-            // blocks past the last reduction-weight index are not fetched: both CTAs' counts
-            const int base = tn * BN;
-            int cnt[2];
-#pragma unroll
-            for (int r2 = 0; r2 < 2; ++r2) {
-              const int left = p.N - (base + r2 * (BN / 2));
-              cnt[r2] = left <= 0 ? 0 : min(BN / 128, (left + 63) / 64);
-            }
-            nblk = cnt[rank];
-            tx = 2u * A_BYTES + (uint32_t)(cnt[0] + cnt[1]) * 8192u;
+            // blocks past the last reduction-weight index are not fetched
+            const int left = p.N - n0;
+            nblk = left <= 0 ? 0 : min(BN / 64, (left + 63) / 64);
+            tx = A_BYTES + (uint32_t)nblk * 8192u;
           }
-          if (leader) mbar_arrive_expect_tx(&full_bar[s], tx);
+          mbar_arrive_expect_tx(&full_bar[s], tx);
           if (AMODE == AM_DENSE) {
-            tma_load_2d_2sm(sa, &tmap_a, &full_bar[s], kb * BK, m0);
+            tma_load_2d(sa, &tmap_a, &full_bar[s], kb * BK, m0);
           } else if (AMODE == AM_DENSE_MN) {
-            // A stored [K][M]: two [64 k][64 m] boxes for this CTA's 128 rows
-            tma_load_2d_2sm(sa, &tmap_a, &full_bar[s], m0, kb * BK);
-            tma_load_2d_2sm(sa + 8192, &tmap_a, &full_bar[s], m0 + 64, kb * BK);
+            // A stored [K][M]: two [64 k][64 m] boxes for the tile's 128 rows
+            tma_load_2d(sa, &tmap_a, &full_bar[s], m0, kb * BK);
+            tma_load_2d(sa + 8192, &tmap_a, &full_bar[s], m0 + 64, kb * BK);
           } else {
-            // this CTA's 128 pixels start at m0; k-block = 64 channels of one filter tap
+            // the tile's 128 pixels start at m0; k-block = 64 channels of one filter tap
             const ConvP& g = p.g;
             const int k0 = kb * BK;
             const int tap = k0 / g.inner, c0 = k0 - tap * g.inner;
@@ -242,15 +157,15 @@ gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
               w0 = ix - (g.KX - 1 - g.PL); h0 = iy - (g.KY - 1 - g.PT);
               ow = g.KX - 1 - kx; oh = g.KY - 1 - ky;
             }
-            tma_load_im2col_2sm(sa, &tmap_a, &full_bar[s], c0, w0, h0, n, (uint16_t)ow, (uint16_t)oh);
+            tma_load_im2col_4d(sa, &tmap_a, &full_bar[s], c0, w0, h0, n, (uint16_t)ow, (uint16_t)oh);
           }
           if (BMODE == BM_K) {
-            tma_load_2d_2sm(sa + A_BYTES, &tmap_b, &full_bar[s], kb * BK, n0);
+            tma_load_2d(sa + A_BYTES, &tmap_b, &full_bar[s], kb * BK, n0);
           } else if (BMODE == BM_MN) {
-            // B stored [K][N] (N contiguous): 64 x 64 boxes, one per 64 columns of this CTA's half
+            // B stored [K][N] (N contiguous): 64 x 64 boxes, one per 64 columns of the tile
 #pragma unroll
-            for (int j = 0; j < BN / 128; ++j)
-              tma_load_2d_2sm(sa + A_BYTES + j * 8192, &tmap_b, &full_bar[s], n0 + j * 64, kb * BK);
+            for (int j = 0; j < BN / 64; ++j)
+              tma_load_2d(sa + A_BYTES + j * 8192, &tmap_b, &full_bar[s], n0 + j * 64, kb * BK);
           } else {
             // conv wgrad: reduction = pixels kb * 64 .., N = (tap, channel); one im2col box of
             // [64 pixels][64 channels] per 64-wide N block
@@ -262,146 +177,109 @@ gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             for (int j = 0; j < nblk; ++j) {
               const int kidx0 = n0 + j * 64;
               const int tap = kidx0 / g.inner, c0 = kidx0 - tap * g.inner;
-              tma_load_im2col_2sm(sa + A_BYTES + j * 8192, &tmap_b, &full_bar[s], c0, w0, h0, n,
-                                  (uint16_t)(tap % g.KX), (uint16_t)(tap / g.KX));
+              tma_load_im2col_4d(sa + A_BYTES + j * 8192, &tmap_b, &full_bar[s], c0, w0, h0, n,
+                                 (uint16_t)(tap % g.KX), (uint16_t)(tap / g.KX));
             }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && lane == 0) {
-      uint32_t it = 0, tcount = 0;
-      for (int t = cid; t < num_tiles; t += nclusters, ++tcount) {
-        const uint32_t acc = tcount & 1, acc_ph = (tcount >> 1) & 1;
-        const int split = t % splits;
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = splits > 1 ? min(total_kb, kb0 + p.kb_per_split) : total_kb;
-        mbar_wait(&tmem_empty_bar[acc], acc_ph ^ 1);      // both CTAs' epilogues drained this buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % NST; const uint32_t ph = (it / NST) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE);
-          const uint32_t sb = sa + A_BYTES;
+    return;
+  }
+
+  // ===================== MMA warpgroups 1, 2: rows 64 (wg - 1) .. + 63 of the tile =============
+  reg_alloc<232>();
+  const int half = wg - 1;
+  const int et = threadIdx.x - 128;                     // 0..255: consumer thread
+  const int wq = warp & 3;                              // warp within the warpgroup
+  const int lr = half * 64 + 16 * wq + (lane >> 2);     // tile row of fragment rows h = 0 (+8 for h = 1)
+  const int cq = 2 * (lane & 3);
+  uint32_t it = 0, chunk_no = 0;
+  float acc[BN / 2];
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    int tm, tn;
+    tile_coords(t / splits, p.tiles_m, p.tiles_n, tm, tn);
+    const int split = t % splits;
+    const int kb0 = split * p.kb_per_split;
+    const int kb1 = splits > 1 ? min(total_kb, kb0 + p.kb_per_split) : total_kb;
+    const int m0 = tm * BM, n0 = tn * BN;
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024)
-                                     : make_smem_desc(sa + k * 32, 16, 1024);
-            const uint64_t db = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024)
-                                     : make_smem_desc(sb + k * 32, 16, 1024);
-            mma_f16_2sm(d_tmem, da, db, IDESC, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          mma_commit_2sm(&empty_bar[s], 3);              // frees the stage in both CTAs
-        }
-        mma_commit_2sm(&tmem_full_bar[acc], 3);          // accumulator ready in both CTAs
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+    for (int kb = kb0; kb < kb1; ++kb, ++it) {
+      const int s = it % NST; const uint32_t ph = (it / NST) & 1;
+      mbar_wait(&full_bar[s], ph);
+      const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE) + half * 8192;
+      const uint32_t sb = smem_u32(tiles + (size_t)s * STAGE) + A_BYTES;
+      wg_fence_regs(acc);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t da = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024)
+                                 : make_smem_desc(sa + k * 32, 16, 1024);
+        const uint64_t db = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024)
+                                 : make_smem_desc(sb + k * 32, 16, 1024);
+        wgmma_bf16<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, 1);
       }
+      wg_commit();
+      wg_fence_regs(acc);
+      wg_wait<1>();                                     // the previous k-block's MMAs retired
+      if (kb > kb0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % NST]);
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue (both CTAs): TMEM -> regs -> smem -> TMA store ============
-    const int ew = warp - 4;                              // TMEM lanes 32 ew .. 32 ew + 31
-    const int et = threadIdx.x - 128;                     // 0..127 = row of the CTA's sub-tile
-    uint32_t tcount = 0, chunk_no = 0;
-    for (int t = cid; t < num_tiles; t += nclusters, ++tcount) {
-      int tm, tn;
-      tile_coords(t / splits, p.tiles_m, p.tiles_n, tm, tn);
-      const int split = t % splits;
-      const int m0 = tm * 2 * BM + (int)rank * BM;
-      const int n0 = tn * BN;
-      // split-K partial s lives at rows [s * M, (s + 1) * M) of the output map: a CTA whose 128
-      // rows lie entirely past M must not store (it would land in the next partial)
-      const bool store_ok = m0 < p.M;
-      const int row0 = split * p.M + m0;
-      const uint32_t acc = tcount & 1, acc_ph = (tcount >> 1) & 1;
-      mbar_wait(&tmem_full_bar[acc], acc_ph);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(ew * 32) << 16) + acc * BN;
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    if (kb1 > kb0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % NST]);
+
+    // ---- epilogue: registers -> swizzled staging chunk -> one TMA store per chunk ----
+    // split-K partial s lives at rows [s * M, (s + 1) * M) of the output map
+    const bool store_ok = m0 < p.M;
+    const int row0 = split * p.M + m0;
+    // (chunk index as a compile-time constant: the accumulator array stays in registers)
+    static_for(std::make_integer_sequence<int, NCHUNK>{}, [&](auto cc_) {
+      constexpr int c = decltype(cc_)::value;
+      uint8_t* buf = epi + (chunk_no & 1) * EPI_BUF;
+      // the TMA store that read this buffer two chunks ago must be done with it
+      if (et == 0) tma_store_wait_read(1);
+      named_bar_sync(1, 256);
+      // this chunk's accumulators (compile-time indices), then a rolled loop over them: the
+      // activation / derivative code is emitted once, not once per element
+      float v[EPI_COLS / 2];
+#pragma unroll
+      for (int k = 0; k < EPI_COLS / 2; ++k) v[k] = acc[c * (EPI_COLS / 2) + k];
 #pragma unroll 1
-      for (int c = 0; c < NCHUNK; ++c, ++chunk_no) {
-        uint8_t* buf = epi + (chunk_no & 1) * EPI_BUF;
-        // the TMA store that read this buffer two chunks ago must be done with it
-        if (et == 0) tma_store_wait_read(1);
-        named_bar_sync(1, 128);
-        uint32_t r[32];
-        uint8_t* rowp = buf + et * 128;
-        const int sw = et & 7;
+      for (int q = 0; q < EPI_COLS / 4; ++q) {
+        const int ii = q >> 1, h = q & 1;               // register pair 4 ii + 2 h (+1)
+        const int cc = ii * 8 + cq;                     // column inside the chunk
+        const int n = n0 + c * EPI_COLS + cc;
+        const int r = lr + 8 * h;
+        const float b0 = (p.bias != nullptr && n < p.N) ? __ldg(p.bias + n) : 0.f;
+        const float b1 = (p.bias != nullptr && n + 1 < p.N) ? __ldg(p.bias + n + 1) : 0.f;
+        float v0 = act_fwd5_fast(p.act, fmaf(v[2 * q], p.alpha, b0));
+        float v1 = act_fwd5_fast(p.act, fmaf(v[2 * q + 1], p.alpha, b1));
+        const int byte = cc * ESZ;
+        uint8_t* dst = buf + r * 128 + (((byte >> 4) ^ (r & 7)) << 4) + (byte & 15);
         if (OUT_F32) {
-          tmem_ld_32x32(trow + c * 32, r);
-          tmem_ld_wait();
-          const int nb = n0 + c * 32;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {                   // 8 chunks of 4 floats = 16 bytes
-            float v[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int n = nb + q * 4 + j;
-              float x = __uint_as_float(r[q * 4 + j]) * p.alpha;
-              if (p.bias != nullptr && n < p.N) x += __ldg(p.bias + n);
-              v[j] = act_fwd5_fast(p.act, x);
-            }
-            *reinterpret_cast<float4*>(rowp + ((q ^ sw) << 4)) = make_float4(v[0], v[1], v[2], v[3]);
-          }
+          *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
         } else {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            tmem_ld_32x32(trow + c * 64 + h * 32, r);
-            tmem_ld_wait();
-            const int nb = n0 + c * 64 + h * 32;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {                 // 4 chunks of 8 bf16 = 16 bytes
-              float v[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int n = nb + q * 8 + j;
-                float x = __uint_as_float(r[q * 8 + j]) * p.alpha;
-                if (p.bias != nullptr && n < p.N) x += __ldg(p.bias + n);
-                v[j] = act_fwd5_fast(p.act, x);
-              }
-              if (p.dmul != nullptr) {
-                // err_input *= f'(x): x has the layout of the output (row pitch ldo)
-                const int row = m0 + et;
-                const int n8 = nb + q * 8;
-                if (row < p.M && n8 + 8 <= p.N) {
-                  float xv[8];
-                  ld8(p.dmul + (long long)row * p.ldo + n8, xv);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) v[j] *= act_deriv(p.dact, 0.f, xv[j]);
-                } else if (row < p.M) {
-#pragma unroll
-                  for (int j = 0; j < 8; ++j)
-                    if (n8 + j < p.N)
-                      v[j] *= act_deriv(p.dact, 0.f, __bfloat162float(p.dmul[(long long)row * p.ldo + n8 + j]));
-                }
-              }
-              st8(reinterpret_cast<__nv_bfloat16*>(rowp + (((h * 4 + q) ^ sw) << 4)), v);
-            }
+          const int row = m0 + r;
+          if (p.dmul != nullptr && row < p.M) {
+            // err_input *= f'(x): x has the layout of the output (row pitch ldo)
+            const __nv_bfloat16* dx = p.dmul + (long long)row * p.ldo + n;
+            if (n < p.N) v0 *= act_deriv(p.dact, 0.f, __bfloat162float(dx[0]));
+            if (n + 1 < p.N) v1 *= act_deriv(p.dact, 0.f, __bfloat162float(dx[1]));
           }
-        }
-        if (c == NCHUNK - 1) {
-          // last TMEM read of this accumulator: hand the buffer back to the MMA issuer (CTA 0)
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_remote(&tmem_empty_bar[acc], 0);
-        }
-        fence_proxy_async_smem();
-        named_bar_sync(1, 128);
-        if (et == 0) {
-          if (store_ok) tma_store_2d(&tmap_c, buf, n0 + c * EPI_COLS, row0);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+          *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
         }
       }
-    }
-    if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+      fence_proxy_async_smem();
+      named_bar_sync(1, 256);
+      if (et == 0) {
+        if (store_ok) tma_store_2d(&tmap_c, buf, n0 + c * EPI_COLS, row0);
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      }
+      ++chunk_no;
+    });
   }
-  tc_fence_before();
-  cluster_sync_all();            // the pair retires together: no remote arrival / smem read outlives a CTA
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, TMEM_COLS);
-  }
+  if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -437,8 +315,7 @@ static int make_map(CUtensorMap* m, const void* ptr, CUtensorMapDataType dt, int
 template <int BN, bool OUT_F32, int AMODE = AM_DENSE, int BMODE = BM_K>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const Params& p,
                   cudaStream_t st) {
-  constexpr int NST = (BN == 256) ? 6 : 8;
-  constexpr int smem = NST * (A_BYTES + (BN / 2) * 128) + 2 * EPI_BUF + 1024;
+  constexpr int smem = pair_stages<BN>() * (A_BYTES + BN * 128) + 2 * EPI_BUF + 1024;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_pair_k<BN, OUT_F32, AMODE, BMODE>,
@@ -446,20 +323,9 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  int sms = 148;
-  {
-    static int cached = 0;
-    if (!cached) {
-      int dev = 0; cudaGetDevice(&dev);
-      cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev);
-      if (cached < 2) cached = 2;
-    }
-    sms = cached;
-  }
   const int tiles = p.tiles_m * p.tiles_n * (p.splits > 1 ? p.splits : 1);
-  int clusters = sms / 2;
-  if (clusters > tiles) clusters = tiles;
-  gemm_pair_k<BN, OUT_F32, AMODE, BMODE><<<dim3(2 * clusters), dim3(256), smem, st>>>(ta, tb, tc, p);
+  const int ctas = tiles < num_sms() ? tiles : num_sms();
+  gemm_pair_k<BN, OUT_F32, AMODE, BMODE><<<dim3(ctas), dim3(THREADS), smem, st>>>(ta, tb, tc, p);
   return (int)cudaGetLastError();
 }
 
@@ -501,7 +367,7 @@ static bool conv_pair_enabled() {
 
 }  // namespace pr
 
-// Convolution forward as an implicit GEMM on the 2-CTA persistent kernel: A = im2col(x) by TMA
+// Convolution forward as an implicit GEMM on the persistent kernel: A = im2col(x) by TMA
 // (im2col mode), B = w_lp [F][ldw] (K = (tap, c) contiguous). out[pix][f] = act(. + bias[f]).
 // Returns 0 when launched, non-zero when the geometry is not served here (caller falls back).
 int launch_conv_fprop_pair(const void* x, const void* w_lp, long long ldw, const float* bias, void* out,
@@ -517,13 +383,13 @@ int launch_conv_fprop_pair(const void* x, const void* w_lp, long long ldw, const
   int r = make_map_im2col(&ta, x, N, H, W, C, -PL, -PT, (OW - 1) * SX + 1 - PL - W,
                           (OH - 1) * SY + 1 - PT - H, SX, SY);
   if (r) return r;
-  r = make_map(&tb, w_lp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, F, ldw, 64, bn / 2);
+  r = make_map(&tb, w_lp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, F, ldw, 64, bn);
   if (r) return r;
   r = make_map(&tc, out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, F, M, F, 64, BM);
   if (r) return r;
   Params p{};
   p.M = M; p.N = F; p.K = K; p.bias = bias; p.act = act; p.alpha = 1.f;
-  p.tiles_m = (M + 2 * BM - 1) / (2 * BM);
+  p.tiles_m = (M + BM - 1) / BM;
   p.tiles_n = (F + bn - 1) / bn;
   p.g = ConvP{H, W, OH, OW, KY, KX, SY, SX, PT, PL, C};
   p.ldo = F;
@@ -555,7 +421,7 @@ int launch_conv_dgrad_pair(const void* err_out, const void* wd_lp, long long ldc
   if (r) return r;
   Params p{};
   p.M = M; p.N = C; p.K = K; p.bias = nullptr; p.act = 0; p.alpha = alpha;
-  p.tiles_m = (M + 2 * BM - 1) / (2 * BM);
+  p.tiles_m = (M + BM - 1) / BM;
   p.tiles_n = (C + bn - 1) / bn;
   p.g = ConvP{H, W, OH, OW, KY, KX, 1, 1, PT, PL, F};
   p.dmul = (const __nv_bfloat16*)dmul; p.dact = dmul ? dact : 0; p.ldo = C;
@@ -566,7 +432,7 @@ int launch_conv_dgrad_pair(const void* err_out, const void* wd_lp, long long ldc
 
 bool conv_pair_on() { return pr::conv_pair_enabled(); }
 
-// Conv weight gradient on the 2-CTA kernel: partials[s][f][kidx] (fp32) = sum over the pixels of
+// Conv weight gradient on the persistent kernel: partials[s][f][kidx] (fp32) = sum over the pixels of
 // split s of err_out[pix][f] * im2col(x)[pix][kidx]. A = err_out^T (stored [pix][F]: MN-major),
 // B = im2col(x) as MN-major [64 pixels][64 channels] boxes (TMA im2col); the output is already in
 // the weights' [F][Kw] layout - no transposed store. F % 128 == 0, C % 64 == 0.
@@ -593,7 +459,7 @@ int launch_conv_wgrad_pair(const void* err_out, const void* x, float* partials, 
   if (r) return r;
   Params p{};
   p.M = F; p.N = Kw; p.K = P; p.bias = nullptr; p.act = 0; p.alpha = 1.f;
-  p.tiles_m = (F + 2 * BM - 1) / (2 * BM);
+  p.tiles_m = (F + BM - 1) / BM;
   p.tiles_n = (Kw + bn - 1) / bn;
   p.splits = splits; p.kb_per_split = kbs;
   p.g = ConvP{H, W, OH, OW, KY, KX, SY, SX, PT, PL, C};
@@ -601,13 +467,13 @@ int launch_conv_wgrad_pair(const void* err_out, const void* x, float* partials, 
   return bn == 256 ? launch<256, true, AM_DENSE_MN, BM_IM2COL_MN>(ta, tb, tc, p, st)
                    : launch<128, true, AM_DENSE_MN, BM_IM2COL_MN>(ta, tb, tc, p, st);
 }
-// splits that give the 74 clusters of the pair kernel ~1 work item each (0: shape not served)
+// splits that give the CTAs of the persistent kernel ~1 work item each (0: shape not served)
 int pair_wgrad_splits(int Kw, int F, int P, int max_splits) {
   using namespace pr;
   if (!conv_pair_enabled() || (Kw % 64) || (F % 128) || F < 128 || Kw < 128 || P < 4096) return 0;
   const int bn = Kw >= 256 ? 256 : 128;
-  const long long tiles = (long long)((F + 255) / 256) * ((Kw + bn - 1) / bn);
-  int s = (int)((74 + tiles - 1) / tiles);
+  const long long tiles = (long long)((F + BM - 1) / BM) * ((Kw + bn - 1) / bn);
+  int s = (int)((num_sms() + tiles - 1) / tiles);
   const int total_kb = (P + BK - 1) / BK;
   if (s > total_kb / 8) s = total_kb / 8;
   if (s > max_splits) s = max_splits;
@@ -632,7 +498,7 @@ int launch_fc_wgrad_pair(const void* err, long long lde, const void* x, long lon
   if (r) return r;
   Params p{};
   p.M = n_out; p.N = n_in; p.K = batch; p.alpha = 1.f;
-  p.tiles_m = (n_out + 2 * BM - 1) / (2 * BM);
+  p.tiles_m = (n_out + BM - 1) / BM;
   p.tiles_n = (n_in + bn - 1) / bn;
   p.splits = 1; p.kb_per_split = (batch + BK - 1) / BK;
   p.ldo = ldo;
@@ -653,14 +519,14 @@ int launch_gemm_pair(const void* a, long long lda, const void* b, long long ldb,
   CUtensorMap ta, tb, tc;
   int r = make_map(&ta, a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, M, lda, 64, BM);
   if (r) return r;
-  r = make_map(&tb, b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, N, ldb, 64, bn / 2);
+  r = make_map(&tb, b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, K, N, ldb, 64, bn);
   if (r) return r;
   r = make_map(&tc, out, out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, esz,
                N, M, ldo, out_f32 ? 32 : 64, BM);
   if (r) return r;
   Params p{};
   p.M = M; p.N = N; p.K = K; p.bias = bias; p.act = act; p.alpha = alpha;
-  p.tiles_m = (M + 2 * BM - 1) / (2 * BM);
+  p.tiles_m = (M + BM - 1) / BM;
   p.tiles_n = (N + bn - 1) / bn;
   p.splits = 1; p.kb_per_split = (K + BK - 1) / BK;
   if (bn == 256) return out_f32 ? launch<256, true>(ta, tb, tc, p, st) : launch<256, false>(ta, tb, tc, p, st);

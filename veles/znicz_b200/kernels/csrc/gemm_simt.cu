@@ -1,5 +1,5 @@
 // Exact-fp32 SIMT implicit-GEMM family (fallback + reference-equivalent baseline path).
-// Used when a shape cannot go through the tcgen05 kernels (TMA alignment: leading dims that are
+// Used when a shape cannot go through the wgmma kernels (TMA alignment: leading dims that are
 // not multiples of 8 elements, e.g. MNIST conv2 F=87 / FC K=791) and for fp32-exact numerics
 // tests. Tile 64x64x16, 256 threads, 4x4 outputs per thread; operands are fetched through
 // functors so dense GEMM (all transposes), conv fprop, conv dgrad and conv wgrad share one
@@ -125,7 +125,7 @@ __global__ void __launch_bounds__(256) gemm_simt_k(AL A, BL B, Epilogue ep, int 
         reinterpret_cast<float*>(ep.out)[(long long)blockIdx.z * ep.split_stride + o] = v;
         continue;
       }
-      v *= ep.alpha;                       // act(alpha * acc + bias), same as the tcgen05 epilogue
+      v *= ep.alpha;                       // act(alpha * acc + bias), same as the wgmma epilogue
       if (ep.bias) v += ep.bias[n];
       v = act_fwd5(ep.act, v);
       if (ep.out_bf16) {

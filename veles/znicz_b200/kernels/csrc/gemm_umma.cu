@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA GEMM family for sm_100a (bf16 operands, fp32 accumulate in TMEM).
+// wgmma / TMA GEMM family for sm_90a (bf16 operands, fp32 accumulate in registers).
 //
 //   D[M, N] = sum_k A[m, k] * B[n, k]      (one 128 x BLOCK_N tile per CTA, optional split-K)
 //
@@ -11,9 +11,10 @@
 //   a temp buffer and calls cuBLAS, /root/reference/conv.py:268-297, gd_conv.py:313-423).
 //   B_TMA_K   B stored [N][K];  B_TMA_MN  B stored [K][N].
 //
-// Warp roles (192 threads): warps 0-3 = gather producers (if any) then epilogue (TMEM -> regs ->
-// bias/activation/alpha-beta -> global); warp 4 = TMA producer; warp 5 = TMEM allocator + the
-// single thread that issues tcgen05.mma and commits to mbarriers. 4-stage smem ring.
+// Warp roles: warpgroup 0 (warps 0-3) issues the wgmma for both 64-row halves of the tile, then
+// runs the epilogue (registers -> shared memory -> bias/activation/alpha-beta -> global); its
+// thread 0 issues the TMA loads. Gather kernels add warpgroup 1 (warps 4-7) as producers.
+// 4-stage smem ring.
 //
 // This covers: FC forward (TMA_K x TMA_K, fused bias+activation), FC dgrad (TMA_K x TMA_MN,
 // alpha/beta), FC wgrad (TMA_MN x TMA_MN), conv fprop (GATHER_K x TMA_K, fused bias+act),
@@ -21,6 +22,8 @@
 // that the fused update kernel sums in fixed order).
 #include "common.cuh"
 #include "umma.cuh"
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <stdlib.h>
 
 namespace zn {
@@ -64,9 +67,6 @@ struct GemmParams {
   // gather source
   const __nv_bfloat16* gsrc; ConvGeomU g; int gather_kind;
   int gK;                      // valid extent of the gathered K (fprop/dgrad) or M (wgrad) index
-  // A_GATHER_K only: consecutive 128-row tiles streamed through ONE pipeline per CTA, each with
-  // its own TMEM columns (amortises prologue / epilogue latency for short-K convolutions)
-  int mt;
   int ktab_n;                  // entries of the gather lookup table (dynamic shared memory)
   int tma_store;               // epilogue: stage the bf16 tile in smem, one TMA store per warp
   int dbg;                     // experiments: 1 = producers skip the gather, 2 = skip the MMAs,
@@ -78,7 +78,6 @@ struct GemmParams {
 // vec mode   : ktab[k / 8] = (ky << 24) | (kx << 16) | c0     (16-byte chunks never straddle a tap)
 // scalar mode: ktab[k]     = (ky << 24) | (kx << 16) | c
 constexpr int KTAB = 4096;
-constexpr int MT_MAX = 4;      // tiles streamed through one CTA (TMEM columns: BLOCK_N * mt <= 512)
 
 struct PixCtx { const __nv_bfloat16* base; int y, x, valid; };
 
@@ -257,6 +256,21 @@ __host__ __device__ constexpr int b_bytes() {
   return B_MODE == B_TMA_K ? BLOCK_N * 128 : ((BLOCK_N + 63) / 64) * 8192;
 }
 
+// 16 e4m3 bytes -> 16 bf16 (exact: 4 significant bits, exponents within range)
+__device__ __forceinline__ void e4m3x16_to_bf16(uint4 v, uint4& lo, uint4& hi) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  uint32_t o[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const __nv_fp8x2_storage_t pr = (__nv_fp8x2_storage_t)((w[j >> 1] >> (16 * (j & 1))) & 0xFFFF);
+    const __half2 h = __half2(__nv_cvt_fp8x2_to_halfraw2(pr, __NV_E4M3));
+    const __nv_bfloat162 b = __float22bfloat162_rn(__half22float2(h));
+    o[j] = *reinterpret_cast<const uint32_t*>(&b);
+  }
+  lo = make_uint4(o[0], o[1], o[2], o[3]);
+  hi = make_uint4(o[4], o[5], o[6], o[7]);
+}
+
 // generic (rare) epilogue element: split-K partials, transposed / fp32 / alpha-beta outputs.
 // Deliberately not inlined: keeps the unrolled epilogue small.
 __device__ __noinline__ void epi_store_slow(const GemmParams& p, int row, int n, float v, int z) {
@@ -279,15 +293,31 @@ __device__ __noinline__ void epi_store_slow(const GemmParams& p, int row, int n,
   }
 }
 
-template <int BLOCK_N, int B_MODE, int STAGES>
+// Threads: warpgroup 0 (warps 0-3) issues the wgmma and runs the epilogue, its thread 0 also issues
+// the TMA loads; gather kernels add warpgroup 1 (warps 4-7) as the implicit-GEMM producers.
+template <int A_MODE>
+__host__ __device__ constexpr int kthreads() {
+  return (A_MODE == A_GATHER_K || A_MODE == A_GATHER_MN) ? 256 : 128;
+}
+// fp32 staging of the accumulator tile for the row-per-thread epilogue: [128][BLOCK_N + 4]
+// (the pad makes the row reads of 8 consecutive threads hit distinct banks)
+template <int BLOCK_N>
+__host__ __device__ constexpr int stage_f32_bytes() {
+  return ((BLOCK_M * (BLOCK_N + 4) * 4) + 1023) & ~1023;
+}
+
+template <int BLOCK_N, int A_MODE, int B_MODE, int STAGES>
 __host__ __device__ constexpr int min_ctas() {
-  return (2 * (STAGES * (A_BYTES + b_bytes<BLOCK_N, B_MODE>()) + 2048) <= 227 * 1024) ? 2 : 1;
+  // the accumulators (BLOCK_N fp32 registers per MMA thread) of a 256-thread gather CTA at
+  // BLOCK_N = 128 do not fit the 128 registers a second CTA would leave
+  return (kthreads<A_MODE>() == 256 && BLOCK_N >= 128) ? 1
+         : ((2 * (STAGES * (A_BYTES + b_bytes<BLOCK_N, B_MODE>()) + 2048) <= 227 * 1024) ? 2 : 1);
 }
 
 // FP8: operands are e4m3 bytes (TMA / TMA, both K-major): the byte geometry of a stage is the
 // same (128-byte swizzled rows), a k-block is 128 elements and every MMA consumes 32 of them.
 template <int BLOCK_N, int A_MODE, int B_MODE, int GKIND, int GVEC, int STAGES, bool FP8 = false>
-__global__ void __launch_bounds__(192, (min_ctas<BLOCK_N, B_MODE, STAGES>()))
+__global__ void __launch_bounds__(kthreads<A_MODE>(), (min_ctas<BLOCK_N, A_MODE, B_MODE, STAGES>()))
 gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
   pdl_trigger();
@@ -296,37 +326,34 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   constexpr bool A_GATHER = (A_MODE == A_GATHER_K || A_MODE == A_GATHER_MN);
   constexpr bool A_MN = (A_MODE == A_TMA_MN || A_MODE == A_GATHER_MN || A_MODE == A_IM2COL_MN);
   constexpr bool B_MN = (B_MODE == B_TMA_MN);
-  constexpr uint32_t TMEM_COLS = BLOCK_N < 32 ? 32 : BLOCK_N;
-  constexpr uint32_t IDESC = FP8 ? make_idesc_e4m3(BLOCK_M, BLOCK_N)
-                                 : make_idesc_bf16(BLOCK_M, BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0);
   constexpr int KBLK = FP8 ? 2 * BLOCK_K : BLOCK_K;      // elements per k-block (128 bytes per row)
   static_assert(!FP8 || (A_MODE == A_TMA_K && B_MODE == B_TMA_K), "fp8: TMA K-major operands only");
+  static_assert(!B_MN || BLOCK_N >= 64, "MN-major B tiles are built from 64-wide swizzle atoms");
+  static_assert(stage_f32_bytes<BLOCK_N>() <= STAGES * STAGE_BYTES, "epilogue staging exceeds the ring");
   constexpr uint32_t TX_BYTES = (A_GATHER ? 0 : A_BYTES) + B_BYTES;
+  constexpr int ACC = BLOCK_N / 2;                        // fp32 registers per 64-row half
+  constexpr int SROW = BLOCK_N + 4;
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tmem_full_bar[MT_MAX];    // one per streamed tile
-  __shared__ uint32_t tmem_base_smem;
 
   // 1024-byte aligned tile area (SWIZZLE_128B atoms are 1024 B)
   uint8_t* tiles = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   // behind the ring: the gather lookup table (only as many entries as this geometry needs - a
-  // fixed-size table cost the BLOCK_N = 64 conv kernels their second CTA per SM) and the tile's
-  // bias slice (the epilogue would otherwise wait on one L2 round trip per 8 columns)
+  // fixed-size table would cost the BLOCK_N = 64 conv kernels their second CTA per SM) and the
+  // tile's bias slice (the epilogue would otherwise wait on one L2 round trip per 8 columns)
   int* const ktab = reinterpret_cast<int*>(tiles + (size_t)STAGES * STAGE_BYTES);
   float* const s_bias = reinterpret_cast<float*>(ktab + ((p.ktab_n + 3) & ~3));
+  // fp8 only: the stage expanded to bf16, A [2][128 rows][128 B] then B [2][BLOCK_N rows][128 B]
+  uint8_t* const cvt_a = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(s_bias + BLOCK_N) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* const cvt_b = cvt_a + 2 * BLOCK_M * 128;
 
   if (p.dbg & 32) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int mt_cfg = (A_MODE == A_GATHER_K && p.mt > 1) ? p.mt : 1;
-  const int m_tiles_total = (p.M + BLOCK_M - 1) / BLOCK_M;
-  const int mtile0 = blockIdx.y * mt_cfg;
-  const int ntiles = min(mt_cfg, m_tiles_total - mtile0);       // tiles this CTA streams (>= 1)
-  const int m0 = mtile0 * BLOCK_M, n0 = blockIdx.x * BLOCK_N;
-  uint32_t tmem_cols = TMEM_COLS;                                 // power of two >= 32
-  while (tmem_cols < (uint32_t)(BLOCK_N * mt_cfg)) tmem_cols <<= 1;
+  const int m0 = blockIdx.y * BLOCK_M, n0 = blockIdx.x * BLOCK_N;
   const int total_kb = (p.K + KBLK - 1) / KBLK;
   const int kb_begin = blockIdx.z * p.k_blocks_per_split;
   const int kb_end = min(total_kb, kb_begin + p.k_blocks_per_split);
@@ -337,16 +364,9 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       mbar_init(&full_bar[s], (A_GATHER ? 128u : 0u) + 1u);
       mbar_init(&empty_bar[s], 1u);
     }
-    for (int j = 0; j < MT_MAX; ++j) mbar_init(&tmem_full_bar[j], 1u);
     fence_barrier_init();
-  }
-  if (warp == 4 && lane == 0) {
     if (!A_GATHER) tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 5) {
-    tmem_alloc(&tmem_base_smem, tmem_cols);
-    tmem_relinquish();
   }
   if (A_GATHER) build_ktab(ktab, p.g, GKIND, p.gK);
   pdl_wait();      // everything above overlapped the previous kernel's tail; global reads start here
@@ -354,133 +374,29 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     const int n = blockIdx.x * BLOCK_N + threadIdx.x;
     s_bias[threadIdx.x] = (p.bias && n < p.N) ? __ldg(p.bias + n) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 4) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      for (int gi = 0; gi < num_kb * ntiles; ++gi) {
-        const int i = gi % num_kb;
-        const int s = gi % STAGES; const uint32_t ph = (gi / STAGES) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        uint8_t* sa = tiles + (size_t)s * STAGE_BYTES;
-        uint8_t* sb = sa + A_BYTES;
-        const int k0 = (kb_begin + i) * KBLK;
-        if (p.dbg & 4) { mbar_arrive(&full_bar[s]); continue; }
-        if (A_MODE == A_IM2COL_MN) {
-          // conv wgrad: tile = [64 pixels (reduction rows)][128 reduction-weight indices] = two
-          // [64 pixels x 64 channels] im2col boxes (one tap each); a block past Kw is skipped
-          const ConvGeomU& g = p.g;
-          const int pix0 = (kb_begin + i) * BLOCK_K;
-          const int q = pix0 % g.OW; const int t2 = pix0 / g.OW;
-          const int pr = t2 % g.OH; const int n = t2 / g.OH;
-          const int w0 = q * g.SX - g.PL, h0 = pr * g.SY - g.PT;
-          const int nblk = (m0 + 64 < p.gK) ? 2 : 1;
-          mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(B_BYTES + nblk * 8192));
-          for (int mb = 0; mb < nblk; ++mb) {
-            const int kidx0 = m0 + mb * 64;
-            const int tap = kidx0 / g.C, c0 = kidx0 - tap * g.C;
-            tma_load_im2col_4d(sa + mb * 8192, &tmap_a, &full_bar[s], c0, w0, h0, n,
-                               (uint16_t)(tap % g.KX), (uint16_t)(tap / g.KX));
-          }
-        } else {
-          mbar_arrive_expect_tx(&full_bar[s], TX_BYTES);
-        }
-        if (A_MODE == A_IM2COL_K) {
-          // conv fprop / stride-1 dgrad: tile rows = pixels m0 .. m0 + 127, k-block = 64
-          // channels of ONE filter tap
-          const ConvGeomU& g = p.g;
-          const int tap = k0 / g.inner, c0 = k0 - tap * g.inner;
-          const int ky = tap / g.KX, kx = tap - ky * g.KX;
-          int w0, h0, n, ow, oh;
-          if (GKIND == G_IM2COL) {
-            const int q = m0 % g.OW; const int t2 = m0 / g.OW;
-            const int pr = t2 % g.OH; n = t2 / g.OH;
-            w0 = q * g.SX - g.PL; h0 = pr * g.SY - g.PT; ow = kx; oh = ky;
-          } else {                                   // dgrad: correlation with the flipped filter
-            const int ix = m0 % g.W; const int t2 = m0 / g.W;
-            const int iy = t2 % g.H; n = t2 / g.H;
-            w0 = ix - (g.KX - 1 - g.PL); h0 = iy - (g.KY - 1 - g.PT);
-            ow = g.KX - 1 - kx; oh = g.KY - 1 - ky;
-          }
-          tma_load_im2col_4d(sa, &tmap_a, &full_bar[s], c0, w0, h0, n, (uint16_t)ow, (uint16_t)oh);
-        } else if (A_MODE == A_TMA_K) {
-          tma_load_2d(sa, &tmap_a, &full_bar[s], k0, m0);
-        } else if (A_MODE == A_TMA_MN) {
-          tma_load_2d(sa, &tmap_a, &full_bar[s], m0, k0);
-          tma_load_2d(sa + 8192, &tmap_a, &full_bar[s], m0 + 64, k0);
-        }
-        if (B_MODE == B_TMA_K) {
-          tma_load_2d(sb, &tmap_b, &full_bar[s], k0, n0);
-        } else {
-#pragma unroll
-          for (int j = 0; j < (BLOCK_N + 63) / 64; ++j)
-            tma_load_2d(sb + j * 8192, &tmap_b, &full_bar[s], n0 + j * 64, k0);
-        }
-      }
-    }
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      for (int gi = 0; gi < num_kb * ntiles; ++gi) {
-        const int i = gi % num_kb;
-        const uint32_t d_tmem = tmem_base + (uint32_t)((gi / num_kb) * BLOCK_N);
-        const int s = gi % STAGES; const uint32_t ph = (gi / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        if (A_GATHER && GVEC == 2) fence_proxy_async_smem();   // LDGSTS data -> async proxy
-        tc_fence_after();
-        const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE_BYTES);
-        const uint32_t sb = sa + A_BYTES;
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) {
-          // K-major: 16 bf16 = 32 B along the swizzled row. MN-major: 16 k-rows = 2 atoms.
-          const uint64_t da = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024)
-                                   : make_smem_desc(sa + k * 32, 16, 1024);
-          const uint64_t db = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024)
-                                   : make_smem_desc(sb + k * 32, 16, 1024);
-          if (!(p.dbg & 2)) {
-            if (FP8) mma_f8(d_tmem, da, db, IDESC, (i > 0 || k > 0) ? 1u : 0u);
-            else mma_f16(d_tmem, da, db, IDESC, (i > 0 || k > 0) ? 1u : 0u);
-          }
-        }
-        mma_commit(&empty_bar[s]);          // smem slot reusable once these MMAs retire
-        if (i == num_kb - 1) mma_commit(&tmem_full_bar[gi / num_kb]);   // this tile's accumulator
-      }
-    }
-  } else {
-    // ============ gather producers, then epilogue (warps 0-3), software-pipelined ============
-    // Round tt issues the gathers of tile tt and then drains the accumulator of tile tt - 1:
-    // with several tiles streamed through one CTA (GemmParams::mt) the epilogue of a tile
-    // overlaps the MMAs of the next one (up to STAGES k-blocks of operands are already in flight),
-    // and the prologue (barriers, TMEM, lookup table) is paid once.
+  if (A_GATHER && threadIdx.x >= 128) {
+    // ===================== gather producers (warpgroup 1) =====================
+    const int t = threadIdx.x - 128;        // 0..127
+    if (A_MODE == A_GATHER_K) {
+      // tile row r = t is GEMM row m0 + t (a pixel); chunks run over the reduction index
+      const int m = m0 + t;
+      const PixCtx ctx = (GKIND == G_IM2COL) ? decode_out_pixel(p.gsrc, p.g, m, p.M)
+                                             : decode_in_pixel(p.gsrc, p.g, m, p.M);
+      if (GVEC == 2) {
+        // asynchronous gather: issue the LDGSTS of a stage as soon as its slot is free; the
+        // stage's full barrier is armed by the copies themselves
 #pragma unroll 1
-    for (int tt = 0; tt <= ntiles; ++tt) {
-    if (A_GATHER && tt < ntiles) {
-      const int t = threadIdx.x;            // 0..127
-      if (A_MODE == A_GATHER_K) {
-        // tile row r = t is GEMM row m0 + t (a pixel); chunks run over the reduction index
-        {
-        const int tj = tt;
-        const int m = m0 + tj * BLOCK_M + t;
-        const int gbase = tj * num_kb;           // position of this tile in the stage sequence
-        const PixCtx ctx = (GKIND == G_IM2COL) ? decode_out_pixel(p.gsrc, p.g, m, p.M)
-                                               : decode_in_pixel(p.gsrc, p.g, m, p.M);
-        if (GVEC == 2) {
-          // asynchronous gather: issue the LDGSTS of a stage as soon as its slot is free; the
-          // stage's full barrier is armed by the copies themselves
-#pragma unroll 1
-          for (int i = 0; i < num_kb; ++i) {
-            const int s = (gbase + i) % STAGES; const uint32_t ph = ((gbase + i) / STAGES) & 1;
-            mbar_wait(&empty_bar[s], ph ^ 1);
-            const uint32_t row_base = smem_u32(tiles + (size_t)s * STAGE_BYTES) + t * 128;
-            if (!(p.dbg & 1))
-              gather_row_async<GKIND>(row_base, t & 7, ktab, p.g, ctx, (kb_begin + i) * BLOCK_K);
-            cp_async_mbar_arrive_noinc(&full_bar[s]);
-          }
-        } else {
+        for (int i = 0; i < num_kb; ++i) {
+          const int s = i % STAGES; const uint32_t ph = (i / STAGES) & 1;
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          const uint32_t row_base = smem_u32(tiles + (size_t)s * STAGE_BYTES) + t * 128;
+          if (!(p.dbg & 1))
+            gather_row_async<GKIND>(row_base, t & 7, ktab, p.g, ctx, (kb_begin + i) * BLOCK_K);
+          cp_async_mbar_arrive_noinc(&full_bar[s]);
+        }
+      } else {
         uint4 v[8], nv[8];
         // software pipeline with ONE load site: iteration i issues the global loads of stage
         // i + 1 and then publishes stage i (whose loads were issued one iteration earlier)
@@ -491,7 +407,7 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             gather_row<GKIND, GVEC>(nv, ktab, p.g, ctx, k0, p.gK);
           }
           if (i >= 0) {
-            const int s = (gbase + i) % STAGES; const uint32_t ph = ((gbase + i) / STAGES) & 1;
+            const int s = i % STAGES; const uint32_t ph = (i / STAGES) & 1;
             mbar_wait(&empty_bar[s], ph ^ 1);
             uint8_t* sa = tiles + (size_t)s * STAGE_BYTES;
 #pragma unroll
@@ -503,29 +419,28 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
           for (int c8 = 0; c8 < 8; ++c8) v[c8] = nv[c8];
         }
-        }
-        }   // tiles of this CTA
-      } else {
-        // A_GATHER_MN (conv wgrad): tile = [64 reduction rows (pixels)][128 m (kidx)];
-        // thread -> reduction row kr = t % 64, 64-wide m block = t / 64 (8 chunks of 8 kidx)
-        const int kr = t & 63, mblk = t >> 6;
-        // only the 64-wide m block that contains index Kw carries the bias "ones" row
-        const int kk0 = m0 + mblk * 64;
-        const bool has_one = p.g.ones != nullptr && kk0 <= p.gK && p.gK < kk0 + 64;
-        if (GVEC == 2) {
+      }
+    } else {
+      // A_GATHER_MN (conv wgrad): tile = [64 reduction rows (pixels)][128 m (kidx)];
+      // thread -> reduction row kr = t % 64, 64-wide m block = t / 64 (8 chunks of 8 kidx)
+      const int kr = t & 63, mblk = t >> 6;
+      // only the 64-wide m block that contains index Kw carries the bias "ones" row
+      const int kk0 = m0 + mblk * 64;
+      const bool has_one = p.g.ones != nullptr && kk0 <= p.gK && p.gK < kk0 + 64;
+      if (GVEC == 2) {
 #pragma unroll 1
-          for (int i = 0; i < num_kb; ++i) {
-            const int s = i % STAGES; const uint32_t ph = (i / STAGES) & 1;
-            mbar_wait(&empty_bar[s], ph ^ 1);
-            const int pix = (kb_begin + i) * BLOCK_K + kr;
-            const PixCtx ctx = decode_out_pixel(p.gsrc, p.g, pix, p.K);
-            const uint32_t row_base =
-                smem_u32(tiles + (size_t)s * STAGE_BYTES) + mblk * 8192 + kr * 128;
-            if (has_one) gather_row_async<G_IM2COL, true>(row_base, kr & 7, ktab, p.g, ctx, kk0);
-            else gather_row_async<G_IM2COL, false>(row_base, kr & 7, ktab, p.g, ctx, kk0);
-            cp_async_mbar_arrive_noinc(&full_bar[s]);
-          }
-        } else {
+        for (int i = 0; i < num_kb; ++i) {
+          const int s = i % STAGES; const uint32_t ph = (i / STAGES) & 1;
+          mbar_wait(&empty_bar[s], ph ^ 1);
+          const int pix = (kb_begin + i) * BLOCK_K + kr;
+          const PixCtx ctx = decode_out_pixel(p.gsrc, p.g, pix, p.K);
+          const uint32_t row_base =
+              smem_u32(tiles + (size_t)s * STAGE_BYTES) + mblk * 8192 + kr * 128;
+          if (has_one) gather_row_async<G_IM2COL, true>(row_base, kr & 7, ktab, p.g, ctx, kk0);
+          else gather_row_async<G_IM2COL, false>(row_base, kr & 7, ktab, p.g, ctx, kk0);
+          cp_async_mbar_arrive_noinc(&full_bar[s]);
+        }
+      } else {
         uint4 v[8], nv[8];
 #pragma unroll 1
         for (int i = -1; i < num_kb; ++i) {
@@ -547,25 +462,180 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
           for (int c8 = 0; c8 < 8; ++c8) v[c8] = nv[c8];
         }
-        }
       }
     }
-    // ===================== epilogue of tile tt - 1 =====================
-    if (tt == 0) continue;
-    const int tj = tt - 1;
-    if (num_kb > 0) {
-      mbar_wait(&tmem_full_bar[tj], 0);
-      tc_fence_after();
+    return;
+  }
+
+  // ===================== warpgroup 0: TMA issue (thread 0), wgmma, epilogue =====================
+  // TMA loads of k-block i into its stage; the slot is free (released by this thread below)
+  auto issue_loads = [&](int i) {
+    const int s = i % STAGES;
+    uint8_t* sa = tiles + (size_t)s * STAGE_BYTES;
+    uint8_t* sb = sa + A_BYTES;
+    const int k0 = (kb_begin + i) * KBLK;
+    if (p.dbg & 4) { mbar_arrive(&full_bar[s]); return; }
+    if (A_MODE == A_IM2COL_MN) {
+      // conv wgrad: tile = [64 pixels (reduction rows)][128 reduction-weight indices] = two
+      // [64 pixels x 64 channels] im2col boxes (one tap each); a block past Kw is skipped
+      const ConvGeomU& g = p.g;
+      const int pix0 = (kb_begin + i) * BLOCK_K;
+      const int q = pix0 % g.OW; const int t2 = pix0 / g.OW;
+      const int pr = t2 % g.OH; const int n = t2 / g.OH;
+      const int w0 = q * g.SX - g.PL, h0 = pr * g.SY - g.PT;
+      const int nblk = (m0 + 64 < p.gK) ? 2 : 1;
+      mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(B_BYTES + nblk * 8192));
+      for (int mb = 0; mb < nblk; ++mb) {
+        const int kidx0 = m0 + mb * 64;
+        const int tap = kidx0 / g.C, c0 = kidx0 - tap * g.C;
+        tma_load_im2col_4d(sa + mb * 8192, &tmap_a, &full_bar[s], c0, w0, h0, n,
+                           (uint16_t)(tap % g.KX), (uint16_t)(tap / g.KX));
+      }
+    } else {
+      mbar_arrive_expect_tx(&full_bar[s], TX_BYTES);
     }
-    // The epilogue runs once per tile, so every instruction of it is an instruction-cache miss:
-    // the former 32-column unrolled version (4-5 K SASS instructions) cost ~10 us per tile on
-    // fetch stalls alone. This one is a rolled loop over 8-column chunks - TMEM loads double
-    // buffered (the next chunk is in flight while this one is stored) - with the output mode
-    // decided once per thread; the loop body is a few hundred instructions, fetched once.
-    enum { EPI_TMA = 0, EPI_BF16 = 1, EPI_RAW_T = 2, EPI_RAW = 3, EPI_SLOW = 4, EPI_NONE = 5,
-           EPI_BIASROW = 6, EPI_F32 = 7 };
-    {
-    const int row = m0 + tj * BLOCK_M + warp * 32 + lane;
+    if (A_MODE == A_IM2COL_K) {
+      // conv fprop / stride-1 dgrad: tile rows = pixels m0 .. m0 + 127, k-block = 64
+      // channels of ONE filter tap
+      const ConvGeomU& g = p.g;
+      const int tap = k0 / g.inner, c0 = k0 - tap * g.inner;
+      const int ky = tap / g.KX, kx = tap - ky * g.KX;
+      int w0, h0, n, ow, oh;
+      if (GKIND == G_IM2COL) {
+        const int q = m0 % g.OW; const int t2 = m0 / g.OW;
+        const int pr = t2 % g.OH; n = t2 / g.OH;
+        w0 = q * g.SX - g.PL; h0 = pr * g.SY - g.PT; ow = kx; oh = ky;
+      } else {                                   // dgrad: correlation with the flipped filter
+        const int ix = m0 % g.W; const int t2 = m0 / g.W;
+        const int iy = t2 % g.H; n = t2 / g.H;
+        w0 = ix - (g.KX - 1 - g.PL); h0 = iy - (g.KY - 1 - g.PT);
+        ow = g.KX - 1 - kx; oh = g.KY - 1 - ky;
+      }
+      tma_load_im2col_4d(sa, &tmap_a, &full_bar[s], c0, w0, h0, n, (uint16_t)ow, (uint16_t)oh);
+    } else if (A_MODE == A_TMA_K) {
+      tma_load_2d(sa, &tmap_a, &full_bar[s], k0, m0);
+    } else if (A_MODE == A_TMA_MN) {
+      tma_load_2d(sa, &tmap_a, &full_bar[s], m0, k0);
+      tma_load_2d(sa + 8192, &tmap_a, &full_bar[s], m0 + 64, k0);
+    }
+    if (B_MODE == B_TMA_K) {
+      tma_load_2d(sb, &tmap_b, &full_bar[s], k0, n0);
+    } else {
+#pragma unroll
+      for (int j = 0; j < (BLOCK_N + 63) / 64; ++j)
+        tma_load_2d(sb + j * 8192, &tmap_b, &full_bar[s], n0 + j * 64, k0);
+    }
+  };
+
+  float acc0[ACC], acc1[ACC];                 // rows 0-63 / 64-127 of the tile
+#pragma unroll
+  for (int j = 0; j < ACC; ++j) { acc0[j] = 0.f; acc1[j] = 0.f; }
+  if (threadIdx.x == 0)
+    for (int i = 0; i < STAGES && i < num_kb; ++i) issue_loads(i);
+#pragma unroll 1
+  for (int i = 0; i < num_kb; ++i) {
+    const int s = i % STAGES; const uint32_t ph = (i / STAGES) & 1;
+    mbar_wait(&full_bar[s], ph);
+    if (A_GATHER && GVEC == 2) fence_proxy_async_smem();   // LDGSTS data -> async proxy
+    const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE_BYTES);
+    const uint32_t sb = sa + A_BYTES;
+    if constexpr (FP8) {
+      // e4m3 wgmma accumulates with fewer mantissa bits than fp32. Every e4m3 value is exact in
+      // bf16, so the stage is expanded to bf16 tiles in shared memory (two 64-element SW128
+      // k-blocks per 128-byte row) and multiplied with bf16 wgmma: fp8 storage and traffic,
+      // fp32 accumulation.
+      const uint8_t* sa8 = tiles + (size_t)s * STAGE_BYTES;
+      const uint8_t* sb8 = sa8 + A_BYTES;
+      for (int q = threadIdx.x; q < (BLOCK_M + BLOCK_N) * 8; q += 128) {
+        const int rr = q >> 3, c = q & 7;
+        const bool is_a = rr < BLOCK_M;
+        const int r = is_a ? rr : rr - BLOCK_M;
+        const uint4 v = *reinterpret_cast<const uint4*>((is_a ? sa8 : sb8) + r * 128 + ((c ^ (r & 7)) << 4));
+        uint4 lo, hi;
+        e4m3x16_to_bf16(v, lo, hi);
+        uint8_t* d = (is_a ? cvt_a : cvt_b) + (c >> 2) * (is_a ? BLOCK_M : BLOCK_N) * 128 + r * 128;
+        const int c2 = (2 * c) & 7;
+        *reinterpret_cast<uint4*>(d + ((c2 ^ (r & 7)) << 4)) = lo;
+        *reinterpret_cast<uint4*>(d + (((c2 + 1) ^ (r & 7)) << 4)) = hi;
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1, 128);
+      if (threadIdx.x == 0) {                  // the e4m3 stage is consumed
+        mbar_arrive(&empty_bar[s]);
+        if (i + STAGES < num_kb) issue_loads(i + STAGES);
+      }
+      wg_fence_regs(acc0); wg_fence_regs(acc1);
+      wg_fence();
+      if (!(p.dbg & 2)) {
+#pragma unroll
+        for (int kb2 = 0; kb2 < 2; ++kb2)
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / 16; ++k) {
+            const uint32_t a0 = smem_u32(cvt_a) + kb2 * BLOCK_M * 128 + k * 32;
+            const uint64_t db = make_smem_desc(smem_u32(cvt_b) + kb2 * BLOCK_N * 128 + k * 32, 16, 1024);
+            wgmma_bf16<BLOCK_N, 0, 0>(acc0, make_smem_desc(a0, 16, 1024), db, 1);
+            wgmma_bf16<BLOCK_N, 0, 0>(acc1, make_smem_desc(a0 + 8192, 16, 1024), db, 1);
+          }
+      }
+      wg_commit();
+      wg_wait<0>();                              // (the next stage overwrites the bf16 tiles)
+      wg_fence_regs(acc0); wg_fence_regs(acc1);
+      continue;
+    }
+    wg_fence_regs(acc0); wg_fence_regs(acc1);
+    wg_fence();
+    if (!(p.dbg & 2)) {
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / 16; ++k) {
+        // K-major: 16 bf16 = 32 B along the swizzled row. MN-major: 16 k-rows = 2 atoms.
+        // The 64-row halves of A are 8192 bytes apart in both layouts.
+        const uint64_t da0 = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024)
+                                  : make_smem_desc(sa + k * 32, 16, 1024);
+        const uint64_t da1 = A_MN ? make_smem_desc(sa + 8192 + k * 2048, 8192, 1024)
+                                  : make_smem_desc(sa + 8192 + k * 32, 16, 1024);
+        const uint64_t db = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024)
+                                 : make_smem_desc(sb + k * 32, 16, 1024);
+        wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc0, da0, db, 1);
+        wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc1, da1, db, 1);
+      }
+    }
+    wg_commit();
+    wg_fence_regs(acc0); wg_fence_regs(acc1);
+    wg_wait<1>();                               // the MMAs of k-block i - 1 have retired
+    if (i > 0 && threadIdx.x == 0) {
+      const int sp = (i - 1) % STAGES;
+      mbar_arrive(&empty_bar[sp]);
+      if (i - 1 + STAGES < num_kb) issue_loads(i - 1 + STAGES);
+    }
+  }
+  wg_wait<0>();
+  wg_fence_regs(acc0); wg_fence_regs(acc1);
+
+  // ===================== epilogue =====================
+  // The accumulator fragments go through shared memory (the ring is idle: every k-block has been
+  // consumed) so that thread t owns row m0 + t; the epilogue proper is then a rolled loop over
+  // 8-column chunks (it runs once per tile, so every instruction of it is an instruction-cache
+  // miss: a short loop body fetched once beats an unrolled one), output mode decided once.
+  float* const stg = reinterpret_cast<float*>(tiles);
+  {
+    const int r0 = 16 * warp + (lane >> 2), cq = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 8; ++i) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        *reinterpret_cast<float2*>(stg + (r0 + 8 * hh) * SROW + 8 * i + cq) =
+            make_float2(acc0[4 * i + 2 * hh], acc0[4 * i + 2 * hh + 1]);
+        *reinterpret_cast<float2*>(stg + (64 + r0 + 8 * hh) * SROW + 8 * i + cq) =
+            make_float2(acc1[4 * i + 2 * hh], acc1[4 * i + 2 * hh + 1]);
+      }
+    }
+  }
+  named_bar_sync(1, 128);
+  enum { EPI_TMA = 0, EPI_BF16 = 1, EPI_RAW_T = 2, EPI_RAW = 3, EPI_SLOW = 4, EPI_NONE = 5,
+         EPI_BIASROW = 6, EPI_F32 = 7 };
+  uint8_t* const tma_stage = tiles + stage_f32_bytes<BLOCK_N>();
+  {
+    const int row = m0 + (int)threadIdx.x;
     const bool raw32 = !p.out_bf16 && p.beta == 0.f && p.alpha == 1.f && !p.bias && p.act == 0;
     float* const rbase = reinterpret_cast<float*>(p.out) +
                          (p.split_stride > 0 ? (long long)blockIdx.z * p.split_stride : 0LL);
@@ -581,7 +651,7 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     else if (raw32 && (p.ldo & 3) == 0 && (reinterpret_cast<uintptr_t>(rbase) & 15) == 0)
       mode = EPI_RAW;
     else mode = EPI_SLOW;
-    const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(tj * BLOCK_N);
+    const float* const srow = stg + threadIdx.x * SROW;
 
     auto emit = [&](const uint32_t (&r)[8], int c0) {
       const int nb = n0 + c0;
@@ -651,7 +721,7 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           return;
         }
         __nv_bfloat16* q = (mode == EPI_TMA)
-            ? reinterpret_cast<__nv_bfloat16*>(tiles + warp * 8192 + lane * (BLOCK_N * 2)) + c0
+            ? reinterpret_cast<__nv_bfloat16*>(tma_stage + warp * 8192 + lane * (BLOCK_N * 2)) + c0
             : reinterpret_cast<__nv_bfloat16*>(p.out) + (long long)row * p.ldo + nb;
         if (mode == EPI_TMA || (nb + 8 <= p.N && (p.ldo & 7) == 0)) {
           st8(q, v);
@@ -683,40 +753,28 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       }
     };
 
-    // rb receives the TMEM load of the next chunk while the current one (ra) is converted and
-    // stored; a single copy of the emit code serves every chunk
-    uint32_t ra[8], rb[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) rb[j] = 0u;
-    if (num_kb > 0) tmem_ld_32x8(trow, rb);
 #pragma unroll 1
     for (int c0 = 0; c0 < BLOCK_N; c0 += 8) {
       if (n0 + c0 >= p.N && mode != EPI_TMA) break;     // chunk beyond the last column
-      if (num_kb > 0) tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 8; ++j) ra[j] = rb[j];
-      if (num_kb > 0 && c0 + 8 < BLOCK_N) tmem_ld_32x8(trow + c0 + 8, rb);
+      uint32_t ra[8];
+      const float4 x0 = *reinterpret_cast<const float4*>(srow + c0);
+      const float4 x1 = *reinterpret_cast<const float4*>(srow + c0 + 4);
+      ra[0] = __float_as_uint(x0.x); ra[1] = __float_as_uint(x0.y);
+      ra[2] = __float_as_uint(x0.z); ra[3] = __float_as_uint(x0.w);
+      ra[4] = __float_as_uint(x1.x); ra[5] = __float_as_uint(x1.y);
+      ra[6] = __float_as_uint(x1.z); ra[7] = __float_as_uint(x1.w);
       emit(ra, c0);
     }
-    if (num_kb > 0) tmem_ld_wait();
     if (p.tma_store) {
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0 && !(p.dbg & 8)) {
         // rows / columns beyond M / N are clipped by the tensor map
-        tma_store_2d(&tmap_c, tiles + warp * 8192, n0, m0 + tj * BLOCK_M + warp * 32);
+        tma_store_2d(&tmap_c, tma_stage + warp * 8192, n0, m0 + warp * 32);
         tma_store_commit_and_wait_read();
       }
       __syncwarp();
     }
-    }
-    }   // rounds (tiles of this CTA)
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
   }
 }
 
@@ -833,18 +891,17 @@ static int launch_stages(const CUtensorMap& ta, const CUtensorMap& tb, const Gem
   }
   const int smem = ring + ((p.ktab_n + 3) & ~3) * 4 + BN * 4;
   CUtensorMap tc = ta;
-  // TMA-store epilogue (smem staging + one tile store per warp) for plain bf16 row-major outputs.
-  // Measured on B200 it is slower than the direct 16-byte stores for these narrow tiles
-  // (CIFAR step 0.270 vs 0.263 ms; conv2 dgrad 25.7 vs 22.6 us): opt-in with ZNICZ_UMMA_TMA_STORE=1.
+  // TMA-store epilogue (smem staging + one tile store per warp) for plain bf16 row-major outputs,
+  // opt-in with ZNICZ_UMMA_TMA_STORE=1 (the default is the direct 16-byte stores).
   static int no_tma_store = -1;
   if (no_tma_store < 0) { const char* e = getenv("ZNICZ_UMMA_TMA_STORE"); no_tma_store = (e && atoi(e)) ? 0 : 1; }
   p.tma_store = 0;
   if (!no_tma_store && p.out_bf16 && p.split_stride == 0 && !p.out_trans && p.beta == 0.f &&
-      (p.ldo % 8) == 0 && ((uintptr_t)p.out & 15) == 0 && 4 * 32 * BN * 2 <= ring - 1024 &&
-      p.mt <= 1) {      // (streamed tiles: the ring is busy with the next tile during the epilogue)
+      (p.ldo % 8) == 0 && ((uintptr_t)p.out & 15) == 0 &&
+      stage_f32_bytes<BN>() + 4 * 8192 <= ring - 1024) {
     if (make_map_out(&tc, p.out, p.N, p.M, p.ldo, BN) == 0) p.tma_store = 1;
   }
-  launch_k(gemm_umma_k<BN, AM, BM, GK, GV, NS>, grid, 192, smem, st, ta, tb, tc, p);
+  launch_k(gemm_umma_k<BN, AM, BM, GK, GV, NS>, grid, kthreads<AM>(), smem, st, ta, tb, tc, p);
   return (int)cudaGetLastError();
 }
 
@@ -858,8 +915,7 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPa
     p.dbg = dbg;
   }
   const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
-  const int mt = (AM == A_GATHER_K && p.mt > 1) ? p.mt : 1;
-  dim3 grid((p.N + BN - 1) / BN, (m_tiles + mt - 1) / mt, splits);
+  dim3 grid((p.N + BN - 1) / BN, m_tiles, splits);
   // Grids that leave one CTA (or none) per SM cannot hide the gather latency by co-residency:
   // give those CTAs an 8-deep ring instead (asynchronous LDGSTS producers only, and only when
   // the K loop is long enough to use it).
@@ -867,20 +923,19 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPa
   if constexpr (deep_ok) {
     const long long ctas = (long long)grid.x * grid.y * grid.z;
     const int kb = p.k_blocks_per_split;
-    // measured neutral on B200 for the CIFAR shapes (the per-k-block cost is not pipeline depth):
     // opt-in with ZNICZ_UMMA_DEEP=1
     static int deep = -1;
     if (deep < 0) { const char* e = getenv("ZNICZ_UMMA_DEEP"); deep = e ? atoi(e) : 0; }
-    if (deep && ctas <= 160 && kb >= 8) return launch_stages<BN, AM, BM, GK, GV, 8>(ta, tb, p, grid, st);
+    if (deep && ctas <= num_sms() && kb >= 8) return launch_stages<BN, AM, BM, GK, GV, 8>(ta, tb, p, grid, st);
   }
   // Short reductions (K <= 4 k-blocks, e.g. a 5x5 first layer on 8 padded channels) in grids of
   // several waves: a 3-stage ring already holds almost the whole K and is small enough for a
-  // third CTA per SM (ncu: these kernels are latency-bound at 15 % warp occupancy).
+  // third CTA per SM (these kernels are latency bound).
   if constexpr (AM == A_GATHER_K && GV == 2 && BN <= 64) {
     const long long ctas = (long long)grid.x * grid.y * grid.z;
     static int s3 = -1;
     if (s3 < 0) { const char* e = getenv("ZNICZ_UMMA_S3"); s3 = e ? atoi(e) : 1; }
-    if (s3 && p.k_blocks_per_split <= 4 && ctas > 2 * 148)
+    if (s3 && p.k_blocks_per_split <= 4 && ctas > 2 * num_sms())
       return launch_stages<BN, AM, BM, GK, GV, 3>(ta, tb, p, grid, st);
   }
   return launch_stages<BN, AM, BM, GK, GV, STAGES_DEFAULT>(ta, tb, p, grid, st);
@@ -913,7 +968,7 @@ int pair_wgrad_splits(int, int, int, int);      // gemm_pair.cu
 
 int umma_pick_splits(int M, int N, int K, int max_splits) {
   {
-    // conv wgrad shapes served by the 2-CTA kernel (gemm_pair.cu) want ~74 work items
+    // conv wgrad shapes served by the persistent kernel (gemm_pair.cu) want ~one work item per SM
     const int sp = pair_wgrad_splits(M, N, K, max_splits);
     if (sp > 0) return sp;
   }
@@ -921,7 +976,7 @@ int umma_pick_splits(int M, int N, int K, int max_splits) {
   if (bn < 64) bn = 64;
   long long tiles = (long long)((M + BLOCK_M - 1) / BLOCK_M) * ((N + bn - 1) / bn);
   int kb = (K + BLOCK_K - 1) / BLOCK_K;
-  int s = (int)((148 + tiles - 1) / tiles);
+  int s = (int)((num_sms() + tiles - 1) / tiles);
   if (s > kb) s = kb;
   if (s > max_splits) s = max_splits;
   return s < 1 ? 1 : s;
@@ -977,7 +1032,7 @@ template <int BN>
 static int launch_fp8_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
                          cudaStream_t st) {
   constexpr int ring = STAGES_DEFAULT * (A_BYTES + b_bytes<BN, B_TMA_K>()) + 1024;
-  constexpr int smem = ring + BN * 4 + 16;
+  constexpr int smem = ring + BN * 4 + 1024 + 2 * (BLOCK_M + BN) * 128;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_umma_k<BN, A_TMA_K, B_TMA_K, 0, 0, STAGES_DEFAULT, true>,
@@ -985,7 +1040,7 @@ static int launch_fp8_bn(const CUtensorMap& ta, const CUtensorMap& tb, const Gem
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  launch_k(gemm_umma_k<BN, A_TMA_K, B_TMA_K, 0, 0, STAGES_DEFAULT, true>, grid, 192, smem, st, ta, tb, ta, p);
+  launch_k(gemm_umma_k<BN, A_TMA_K, B_TMA_K, 0, 0, STAGES_DEFAULT, true>, grid, 128, smem, st, ta, tb, ta, p);
   return (int)cudaGetLastError();
 }
 // a [M][lda] e4m3, b [N][ldb] e4m3 (both K-major, ld % 16 == 0); alpha carries 1/(scale_a*scale_b)
@@ -1004,7 +1059,7 @@ int launch_gemm_fp8(const void* a, long long lda, const void* b, long long ldb, 
   p.k_blocks_per_split = (K + 2 * BLOCK_K - 1) / (2 * BLOCK_K);
   p.out = out; p.out_bf16 = out_bf16; p.ldo = ldo; p.out_trans = 0;
   p.bias = bias; p.act = act; p.alpha = alpha; p.beta = 0.f; p.split_stride = 0;
-  p.gather_kind = G_NONE; p.mt = 1;
+  p.gather_kind = G_NONE;
   dim3 grid((N + bn - 1) / bn, (M + BLOCK_M - 1) / BLOCK_M, 1);
   switch (bn) {
     case 16: return launch_fp8_bn<16>(ta, tb, p, grid, st);
@@ -1018,24 +1073,6 @@ static ConvGeomU geom(int N, int H, int W, int C, int OH, int OW, int F, int KY,
                       int PT, int PL, int vec) {
   ConvGeomU g{N, H, W, C, OH, OW, F, KY, KX, SY, SX, PT, PL, vec, 0, KY * KX, 0};
   return g;
-}
-// Tiles streamed per CTA (GemmParams::mt): only when the grid would otherwise need more than one
-// wave at two CTAs per SM, and never so many that fewer than one CTA per SM remains.
-static int pick_mt(int M, int N, int bn) {
-  const long long m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-  const long long n_tiles = (N + bn - 1) / bn;
-  // Measured on B200 (CIFAR step): with the epilogue of tile t overlapping the MMAs of tile t + 1
-  // (the "rounds" loop of the kernel) streaming 2 or 4 tiles per CTA is neutral (444.9 K / 445.3 K
-  // vs 442.7-447 K images/s); before that overlap existed it was slower (conv1 fprop 36 us vs
-  // 32.7 us). Independent CTAs already hide each other's prologues, so the mode stays opt-in
-  // (ZNICZ_UMMA_MT=2|4); a persistent scheduler with TMEM double buffering is the round-2 form.
-  static int forced = -1;
-  if (forced < 0) { const char* e = getenv("ZNICZ_UMMA_MT"); forced = e ? atoi(e) : 1; }
-  int mt = 1;
-  while (mt < forced && mt < 4 && bn * mt * 2 <= 256 && (m_tiles * n_tiles) / (mt * 2) >= 148 &&
-         m_tiles * n_tiles > 296)
-    mt *= 2;
-  return mt;
 }
 // Enable the tap-mode gather when the inner (channel) extent tiles a 64-wide reduction block.
 static bool set_tap_mode(ConvGeomU& g, int inner, bool dgrad) {
@@ -1065,7 +1102,7 @@ int launch_conv_fprop_umma(const void* x, const void* w_lp, long long ldw, const
   if ((ldw % 8) || ((uintptr_t)w_lp & 15) || ((uintptr_t)x & 15)) return -3;
   if (out_bf16 && launch_conv_fprop_pair(x, w_lp, ldw, bias, out, N, H, W, C, OH, OW, F, KY, KX, SY, SX, PT,
                                          PL, act, st) == 0) {
-    ++g_pair_conv_launches;        // large layer: 2-CTA persistent kernel, A by TMA im2col
+    ++g_pair_conv_launches;        // large layer: persistent kernel, A by TMA im2col
     return 0;
   }
   int Kw = KY * KX * C;
@@ -1082,13 +1119,12 @@ int launch_conv_fprop_umma(const void* x, const void* w_lp, long long ldw, const
   p.bias = bias; p.act = act; p.alpha = 1.f; p.beta = 0.f; p.split_stride = 0;
   p.gsrc = (const __nv_bfloat16*)x; p.g = geom(N, H, W, C, OH, OW, F, KY, KX, SY, SX, PT, PL, C % 8 == 0);
   p.gather_kind = G_IM2COL; p.gK = Kw;
-  p.mt = pick_mt(p.M, p.N, bn);
   if (C % 64 == 0 && im2col_tma_enabled()) {
     // A operand by TMA im2col: window bases -PL .. W + upper_w, OW x OH of them
     CUtensorMap ti;
     if (make_map_im2col(&ti, x, N, H, W, C, -PL, -PT, (OW - 1) * SX + 1 - PL - W,
                         (OH - 1) * SY + 1 - PT - H, SX, SY, BLOCK_M) == 0) {
-      p.g.inner = C; p.mt = 1;
+      p.g.inner = C;
       ++g_im2col_launches;
       return launch_bn<A_IM2COL_K, B_TMA_K, G_IM2COL, 0>(bn, ti, tb, p, 1, st);
     }
@@ -1130,7 +1166,6 @@ int launch_conv_dgrad_umma(const void* err_out, const void* wd_lp, long long ldc
   p.g = geom(N, H, W, C, OH, OW, F, KY, KX, SY, SX, PT, PL, F % 8 == 0);
   p.gather_kind = G_DGRAD; p.gK = Kd;
   p.dmul = (const __nv_bfloat16*)dmul; p.dact = dmul ? dact : 0;
-  p.mt = pick_mt(p.M, p.N, bn);
   if (F % 64 == 0 && SY == 1 && SX == 1 && im2col_tma_enabled()) {
     // unit stride: dgrad is a correlation of err_out with the flipped filter; W x H window bases
     // starting at -(K - 1 - pad) over the [N][OH][OW][F] tensor
@@ -1138,7 +1173,7 @@ int launch_conv_dgrad_umma(const void* err_out, const void* wd_lp, long long ldc
     const int lw = -(KX - 1 - PL), lh = -(KY - 1 - PT);
     if (make_map_im2col(&ti, err_out, N, OH, OW, F, lw, lh, W + lw - OW, H + lh - OH, 1, 1,
                         BLOCK_M) == 0) {
-      p.g.inner = F; p.mt = 1;
+      p.g.inner = F;
       ++g_im2col_launches;
       return launch_bn<A_IM2COL_K, B_TMA_MN, G_DGRAD, 0>(bn, ti, tb, p, 1, st);
     }
@@ -1182,9 +1217,8 @@ int launch_conv_wgrad_umma(const void* err_out, const void* x, float* partials, 
   p.gather_kind = G_IM2COL; p.gK = Kw;
   static int wg_tma = -1;
   if (wg_tma < 0) { const char* e = getenv("ZNICZ_IM2COL_TMA_WGRAD"); wg_tma = (e && atoi(e)) ? 1 : 0; }
-  // (measured on the AlexNet shapes: 224-231 vs 231-249 TFLOP/s for the LDGSTS gather, which
-  // also delivers the bias row - so the single-CTA TMA form is opt-in; large layers take the
-  // 2-CTA kernel above)
+  // (the LDGSTS gather also delivers the bias row, so the single-CTA TMA form is opt-in; large
+  // layers take the persistent kernel above)
   if (wg_tma && C % 64 == 0 && im2col_tma_enabled()) {
     // im2col operand by TMA, 64 pixels x 64 channels per box (no "ones" row here: the caller
     // computes the bias gradient with the column-sum kernel when this returns 0)

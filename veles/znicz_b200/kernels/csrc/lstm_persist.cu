@@ -1,4 +1,4 @@
-// Persistent LSTM sequence kernels (sm_100a): the whole time loop of an LSTM layer in ONE launch.
+// Persistent LSTM sequence kernels (sm_90a): the whole time loop of an LSTM layer in ONE launch.
 //
 //   forward   z_t = [x_t | h_{t-1}] . W^T + b,  (i, f, g, o) = act(z_t),  c_t = i g + f c_{t-1},
 //             h_t = o * A tanh(B c_t)                         (/root/reference/lstm.py:75-143)
@@ -11,25 +11,24 @@
 // forward
 // * CTA c owns hidden units [32 c, 32 c + 32): the 4 x 32 rows of W of their gates stay RESIDENT
 //   in shared memory for the whole sequence (96 KB at I = 128, H = 256), loaded once by TMA;
-// * per step ONE tcgen05 accumulation D[128 x 128] in TMEM (double buffered): the x part (K = I,
-//   no recurrence) is issued a step ahead, the h part (K = H) the moment h_{t-1} has arrived;
-// * the cell math runs in the epilogue straight from TMEM (thread = batch row x 16 units), c_t
-//   lives in registers across the steps;
+// * per step one wgmma accumulation D[R x 128] in registers (two MMA warpgroups of 64 rows): the
+//   x part (K = I, no recurrence) is issued first and runs while the h part (K = H) waits for
+//   h_{t-1};
+// * the cell math runs straight on the accumulator fragment: the 4 gate columns of a unit sit in
+//   the same thread (thread = 2 batch rows x 8 units), c_t lives in registers across the steps;
 // * the cluster exchanges h_t through L2: bf16 stores into the [x | h] operand of step t + 1 ->
-//   fence.proxy.async -> barrier.cluster (release / acquire) -> TMA loads. (Measured
-//   alternatives, tools/lstm_probe.py: pushing h into the 8 peers with st.shared::cluster costs
-//   64 KB of DSMEM stores per CTA and step at ~21 B/clk - 3x slower than the 64 KB TMA load.)
+//   fence.proxy.async -> barrier.cluster (release / acquire) -> TMA loads.
 // * critical path first: h is stored and announced BEFORE the state for the backward pass is
 //   written; that state (gates as bf16, c as fp32) uses a lane-major private layout in which every
-//   warp-wide store is one contiguous 512-byte piece (row-major 64-byte pieces cost 5.9 of 9.2 us
-//   per step in the first version).
+//   warp-wide store is one contiguous 512-byte piece.
 // backward
 // * dz_t of the CTA's own units goes from the epilogue straight into its own A operand (swizzled
 //   smem) and is multiplied by the resident W_h rows of those gates: P_c[R x H] = dz_t[:, own] .
 //   W_h[own, :] (K = 128, N = H, one accumulation per step);
-// * the partial sums are reduce-scattered through L2 as bf16 in the same lane-major layout
-//   (coalesced on both sides) under barrier.cluster; CTA d adds the H / 32 pieces of its units in
-//   fp32 -> dh_{t-1}; dc lives in registers.
+// * the partial sums are reduce-scattered through L2 as bf16 (the owner of a unit has the same
+//   fragment rows as every producer of it: 32 contiguous bytes per thread and owner) under
+//   barrier.cluster; CTA d adds the H / 32 pieces of its units in fp32 -> dh_{t-1}; dc lives in
+//   registers.
 // Launch-count: 2 (+ the W_h^T permutation) instead of ~5 T.
 #include "common.cuh"
 #include "umma.cuh"
@@ -42,9 +41,8 @@ namespace lp {
 
 constexpr int BM = 128;
 constexpr int U = 32;                   // hidden units per CTA
-constexpr int UH = 16;                  // ... per epilogue thread (two warps share a TMEM lane quarter)
 constexpr int NG = 4 * U;               // gate columns per CTA
-constexpr int THREADS = 320;            // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
+constexpr int THREADS = 384;            // warpgroup 0 TMA, warpgroups 1, 2 MMA + cell math
 constexpr int SVEC = 12;                // 16-byte vectors per thread and step in the private state layout
 
 __device__ __forceinline__ uint32_t cl_rank() {
@@ -80,10 +78,21 @@ __device__ __forceinline__ uint32_t sw128(int r, int ch) {
   return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((ch ^ (r & 7)) << 4));
 }
 
+// Consumer-thread geometry shared by both kernels and the state unpacker: consumer thread
+// tid = threadIdx.x - 128 (warp ew = tid / 32 of warpgroup wgc = ew / 4) owns batch rows
+// rA = 64 wgc + 16 (ew % 4) + lane / 4 and rA + 8 and, of the CTA's 32 units, 8 ii + 2 (lane % 4) + e
+// (ii < 4, e < 2): the wgmma accumulator fragment. Its 16 (row, unit) "slots" are numbered
+// s = 4 ii + 2 h + e (h: row rA + 8 h), so gate g of slot s is accumulator register 16 g + s.
+__device__ __forceinline__ int slot_row(int ew, int lane, int s) {
+  return (ew >> 2) * 64 + 16 * (ew & 3) + (lane >> 2) + 8 * ((s >> 1) & 1);
+}
+__device__ __forceinline__ int slot_unit(int lane, int s) { return 8 * (s >> 2) + 2 * (lane & 3) + (s & 1); }
+
 // Private state layout (forward -> backward), 16-byte vectors:
-//   ((t * n_ctas + cta) * 8 + epilogue warp) * SVEC + v) * 32 + lane
-// v = 0,1: input gate of the thread's 16 units as bf16, 2,3 forget, 4,5 memory maker, 6,7 output gate,
-// 8..11: cell state fp32. Every warp-wide access is one contiguous 512-byte piece.
+//   ((t * n_ctas + cta) * 8 + consumer warp) * SVEC + v) * 32 + lane
+// v = 2 g + j: gate g (input, forget, memory maker, output) of slots 8 j .. 8 j + 7 as bf16;
+// v = 8 + j: cell state of slots 4 j .. 4 j + 3 as fp32. Every warp-wide access is one contiguous
+// 512-byte piece.
 __device__ __forceinline__ size_t state_idx(int t, int n_ctas, int cta, int ew, int v, int lane) {
   return ((((size_t)t * n_ctas + cta) * 8 + ew) * SVEC + v) * 32 + lane;
 }
@@ -104,24 +113,21 @@ lstm_fwd_k(const __grid_constant__ CUtensorMap t_xh, const __grid_constant__ CUt
   uint8_t* sW = sm;                                   // (KX + KH) blocks x [NG rows][128 B]
   uint8_t* sX = sW + (size_t)(KX + KH) * NG * 128;    // 2 stages x KX blocks x [128 rows][128 B]
   uint8_t* sH = sX + (size_t)2 * KX * BM * 128;       // KH blocks x [128 rows][128 B]: h_{t-1}
-  __shared__ __align__(8) uint64_t w_full, x_full[2], x_empty[2], h_full, acc_full[2], acc_empty[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t w_full, x_full[2], x_empty[2], h_full;
   __shared__ float s_bias[NG];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = (int)cl_rank();
-  const int csize = p.H / U;
   const int T = p.T, B = p.B, I = p.I, H = p.H, R = p.R;
+  const int csize = H / U;
   const int row0 = (blockIdx.x / csize) * R;           // first batch row of this cluster
   const uint32_t tile_bytes = (uint32_t)(R * 128);     // one k-block of R rows
+  const int nwg = R > 64 ? 2 : 1;                      // MMA warpgroups with batch rows
 
   if (threadIdx.x == 0) {
     mbar_init(&w_full, 1);
     mbar_init(&h_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&x_full[s], 1); mbar_init(&x_empty[s], 1);
-      mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], (uint32_t)(2 * (R / 32)));
-    }
+    for (int s = 0; s < 2; ++s) { mbar_init(&x_full[s], 1); mbar_init(&x_empty[s], (uint32_t)nwg); }
     fence_barrier_init();
     tma_prefetch_desc(&t_xh);
     tma_prefetch_desc(&t_w);
@@ -130,16 +136,12 @@ lstm_fwd_k(const __grid_constant__ CUtensorMap t_xh, const __grid_constant__ CUt
     const int g = threadIdx.x / U, j = threadIdx.x % U;
     s_bias[threadIdx.x] = p.bias ? p.bias[g * H + c * U + j] : 0.f;
   }
-  if (warp == 1) { tmem_alloc(&tmem_slot, 2 * NG); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-  constexpr uint32_t IDESC = make_idesc_bf16(BM, NG, 0, 0);
 
-  if (warp == 0) {
-    // ---------------------------------------------------------------- TMA producer
-    if (lane == 0) {
+  if (warp < 4) {
+    // ---------------------------------------------------------------- producer warpgroup
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(&w_full, (uint32_t)((KX + KH) * NG * 128));
       for (int kb = 0; kb < KX + KH; ++kb)
         for (int g = 0; g < 4; ++g)
@@ -152,7 +154,7 @@ lstm_fwd_k(const __grid_constant__ CUtensorMap t_xh, const __grid_constant__ CUt
     }
     for (int t = 1; t < T; ++t) {
       cl_arrive(); cl_wait();                         // every CTA's slice of h_{t-1} is in xh[t]
-      if (lane == 0) {
+      if (threadIdx.x == 0) {
         fence_proxy_async_all();
         mbar_arrive_expect_tx(&h_full, KH * tile_bytes);
         for (int kb = 0; kb < KH; ++kb)
@@ -167,93 +169,74 @@ lstm_fwd_k(const __grid_constant__ CUtensorMap t_xh, const __grid_constant__ CUt
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    auto x_part = [&](int t) {
-      const int s = t & 1;
-      mbar_wait(&x_full[s], (t >> 1) & 1);
-      if (t >= 2) mbar_wait(&acc_empty[s], ((t >> 1) - 1) & 1);
-      tc_fence_after();
-      const uint32_t d = tmem_base + (uint32_t)(s * NG);
-      for (int kb = 0; kb < KX; ++kb) {
-        const uint32_t sa = smem_u32(sX + (size_t)(s * KX + kb) * BM * 128);
-        const uint32_t sb = smem_u32(sW + (size_t)kb * NG * 128);
+  } else {
+    // ------------------------------------------- MMA warpgroups: z_t = [x_t | h_{t-1}] . W^T, cell math
+    reg_alloc<232>();
+    const int tid = threadIdx.x - 128, ew = tid >> 5, wgc = ew >> 2;
+    const bool mma = wgc < nwg;                        // warpgroup-uniform
+    const int n_ctas = gridDim.x;
+    float cst[16];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          mma_f16(d, make_smem_desc(sa + k * 32, 16, 1024), make_smem_desc(sb + k * 32, 16, 1024), IDESC,
-                  (kb > 0 || k > 0) ? 1u : 0u);
-      }
-      mma_commit(&x_empty[s]);
-    };
-    if (lane == 0) {
-      mbar_wait(&w_full, 0);
-      x_part(0);
-      mma_commit(&acc_full[0]);                       // h_{-1} = 0: step 0 is the x part alone
-      if (T > 1) x_part(1);
-    }
-    __syncwarp();
-    for (int t = 1; t < T; ++t) {
-      cl_arrive(); cl_wait();
-      if (lane == 0) {
-        mbar_wait(&h_full, (t - 1) & 1);
-        if (p.dbg && blockIdx.x == 0) p.dbg[t * 8 + 2] = clock64();
-        tc_fence_after();
-        const uint32_t d = tmem_base + (uint32_t)((t & 1) * NG);
-        for (int kb = 0; kb < KH; ++kb) {
-          const uint32_t sa = smem_u32(sH + (size_t)kb * BM * 128);
-          const uint32_t sb = smem_u32(sW + (size_t)(KX + kb) * NG * 128);
+    for (int j = 0; j < 16; ++j) cst[j] = 0.f;
+    if (mma) mbar_wait(&w_full, 0);
+    for (int t = 0; t < T; ++t) {
+      float gi[16], gf[16], gg[16], go[16];
+      if (mma) {
+        float acc[NG / 2];
+        const int s = t & 1;
+        mbar_wait(&x_full[s], (t >> 1) & 1);
+        if (p.dbg && blockIdx.x == 0 && tid == 0) p.dbg[t * 8 + 2] = clock64();
+        wg_fence();
+        // x part (no recurrence), then the h part once h_{t-1} has arrived
+        for (int kb = 0; kb < KX; ++kb) {
+          const uint32_t sa = smem_u32(sX + (size_t)(s * KX + kb) * BM * 128) + wgc * 8192;
+          const uint32_t sb = smem_u32(sW + (size_t)kb * NG * 128);
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-            mma_f16(d, make_smem_desc(sa + k * 32, 16, 1024), make_smem_desc(sb + k * 32, 16, 1024), IDESC, 1u);
+            wgmma_bf16<NG, 0, 0>(acc, make_smem_desc(sa + k * 32, 16, 1024), make_smem_desc(sb + k * 32, 16, 1024),
+                                 (kb > 0 || k > 0) ? 1 : 0);
         }
-        mma_commit(&acc_full[t & 1]);
-        if (t + 1 < T) x_part(t + 1);                 // no recurrence in it: runs under the epilogue
-      }
-      __syncwarp();
-    }
-  } else {
-    // ---------------------------------------------------------------- epilogue: cell math
-    const int ew = warp - 2;
-    const int q = warp & 3, half = ew >> 2;
-    const int r = q * 32 + lane;
-    const int b = row0 + r;
-    const bool active = q * 32 < R;                    // warp-uniform
-    const bool valid = active && b < B;
-    const int j0 = c * U + half * UH;                  // first hidden unit of this thread
-    const int n_ctas = gridDim.x;
-    float cst[UH];
+        wg_commit();
+        if (t > 0) {
+          mbar_wait(&h_full, (t - 1) & 1);
+          for (int kb = 0; kb < KH; ++kb) {
+            const uint32_t sa = smem_u32(sH + (size_t)kb * BM * 128) + wgc * 8192;
+            const uint32_t sb = smem_u32(sW + (size_t)(KX + kb) * NG * 128);
 #pragma unroll
-    for (int j = 0; j < UH; ++j) cst[j] = 0.f;
-    for (int t = 0; t < T; ++t) {
-      float gi[UH], gf[UH], gg[UH], go[UH], hv[UH];
-      if (active) {
-        mbar_wait(&acc_full[t & 1], (t >> 1) & 1);
-        if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) p.dbg[t * 8 + 3] = clock64();
-        tc_fence_after();
-        uint32_t z[4][UH];
-        const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((t & 1) * NG + half * UH);
+            for (int k = 0; k < 4; ++k)
+              wgmma_bf16<NG, 0, 0>(acc, make_smem_desc(sa + k * 32, 16, 1024), make_smem_desc(sb + k * 32, 16, 1024), 1);
+          }
+          wg_commit();
+        }
+        wg_wait<0>();
+        wg_fence_regs(acc);
+        if ((tid & 127) == 0) mbar_arrive(&x_empty[s]);
+        if (p.dbg && blockIdx.x == 0 && tid == 0) p.dbg[t * 8 + 3] = clock64();
+        float hv[16];
 #pragma unroll
-        for (int g = 0; g < 4; ++g) tmem_ld_32x16(ta + g * U, z[g]);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[t & 1]);
-#pragma unroll
-        for (int j = 0; j < UH; ++j) {
-          const int n = half * UH + j;
-          gi[j] = sigm_fast(__uint_as_float(z[0][j]) + s_bias[n]);
-          gf[j] = sigm_fast(__uint_as_float(z[1][j]) + s_bias[U + n]);
-          gg[j] = 1.7159f * tanh_fast(0.6666f * (__uint_as_float(z[2][j]) + s_bias[2 * U + n]));
-          go[j] = sigm_fast(__uint_as_float(z[3][j]) + s_bias[3 * U + n]);
+        for (int j = 0; j < 16; ++j) {
+          const int n = slot_unit(lane, j);
+          gi[j] = sigm_fast(acc[j] + s_bias[n]);
+          gf[j] = sigm_fast(acc[16 + j] + s_bias[U + n]);
+          gg[j] = 1.7159f * tanh_fast(0.6666f * (acc[32 + j] + s_bias[2 * U + n]));
+          go[j] = sigm_fast(acc[48 + j] + s_bias[3 * U + n]);
           cst[j] = fmaf(gi[j], gg[j], gf[j] * cst[j]);
           hv[j] = go[j] * (1.7159f * tanh_fast(0.6666f * cst[j]));
         }
-        if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) p.dbg[t * 8 + 4] = clock64();
+        if (p.dbg && blockIdx.x == 0 && tid == 0) p.dbg[t * 8 + 4] = clock64();
         // critical path first: h_t into the operand of step t + 1 (also the wgrad operand)
-        if (valid) {
-          uint4* np = reinterpret_cast<uint4*>(p.xh + ((size_t)(t + 1) * B + b) * (I + H) + I + j0);
-          np[0] = pack8(hv);
-          np[1] = pack8(hv + 8);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = slot_row(ew, lane, 2 * h);
+          const int b = row0 + r;
+          if (r < R && b < B) {
+            __nv_bfloat16* hp = p.xh + ((size_t)(t + 1) * B + b) * (I + H) + I + c * U;
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii) {
+              const int j = 4 * ii + 2 * h;
+              *reinterpret_cast<__nv_bfloat162*>(hp + slot_unit(lane, j)) = __floats2bfloat162_rn(hv[j], hv[j + 1]);
+            }
+          }
         }
       }
       if (t < T - 1) {
@@ -261,8 +244,8 @@ lstm_fwd_k(const __grid_constant__ CUtensorMap t_xh, const __grid_constant__ CUt
         if (t > 0) cl_wait();                         // close phase t - 1 before arriving on phase t
         cl_arrive();
       }
-      if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) p.dbg[t * 8 + 5] = clock64();
-      if (active) {
+      if (p.dbg && blockIdx.x == 0 && tid == 0) p.dbg[t * 8 + 5] = clock64();
+      if (mma) {
         // off the critical path: state for the backward pass, one 512-byte piece per warp store
         uint4* sp = p.state + state_idx(t, n_ctas, blockIdx.x, ew, 0, lane);
         sp[0 * 32] = pack8(gi); sp[1 * 32] = pack8(gi + 8);
@@ -274,13 +257,10 @@ lstm_fwd_k(const __grid_constant__ CUtensorMap t_xh, const __grid_constant__ CUt
           sp[(8 + v) * 32] = make_uint4(__float_as_uint(cst[4 * v]), __float_as_uint(cst[4 * v + 1]),
                                         __float_as_uint(cst[4 * v + 2]), __float_as_uint(cst[4 * v + 3]));
       }
-      if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) p.dbg[t * 8 + 6] = clock64();
+      if (p.dbg && blockIdx.x == 0 && tid == 0) p.dbg[t * 8 + 6] = clock64();
     }
     if (T > 1) cl_wait();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 2 * NG); }
 }
 
 struct BwdP {
@@ -289,93 +269,56 @@ struct BwdP {
   long long lde;              // row pitch of err (elements)
   int seq;
   const uint4* state;         // private layout written by lstm_fwd_k
-  uint4* part;                // [2][n_ctas][8 warps][H / 16 vectors][32 lanes]: bf16 partial sums
+  uint4* part;                // [2][n_ctas][H / 32 owners][256 threads][2]: bf16 partial sums
   __nv_bfloat16* dz;          // [T][B][4H]
 };
 
+template <int HN>
 __global__ void __launch_bounds__(THREADS, 1)
 lstm_bwd_k(const __grid_constant__ CUtensorMap t_whp, BwdP p) {
+  constexpr int H = HN, CS = HN / U;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int H = p.H, T = p.T, B = p.B, R = p.R;
-  const int csize = H / U;
+  const int T = p.T, B = p.B, R = p.R;
   uint8_t* sB = sm;                                   // 2 k-blocks x [H rows][128 B]: W_h rows of own gates
   uint8_t* sA = sB + (size_t)2 * H * 128;             // 2 k-blocks x [128 rows][128 B]: own dz_t
-  __shared__ __align__(8) uint64_t b_full, a_ready, acc_full;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t b_full;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = (int)cl_rank();
-  const int row0 = (blockIdx.x / csize) * R;
-  const uint32_t tcols = H <= 64 ? 64u : (H <= 128 ? 128u : 256u);
-  const int NV = H / 16;                              // partial vectors (8 bf16) per thread: H / 2 columns
+  const int row0 = (blockIdx.x / CS) * R;
   const int n_ctas = gridDim.x;
-  const size_t part_buf = (size_t)n_ctas * 8 * NV * 32;
+  const size_t part_buf = (size_t)n_ctas * CS * 256 * 2;
+  const int nwg = R > 64 ? 2 : 1;
 
   if (threadIdx.x == 0) {
     mbar_init(&b_full, 1);
-    mbar_init(&a_ready, (uint32_t)(2 * (R / 32)));
-    mbar_init(&acc_full, 1);
     fence_barrier_init();
     tma_prefetch_desc(&t_whp);
   }
-  if (warp == 1) { tmem_alloc(&tmem_slot, tcols); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-  const uint32_t idesc = make_idesc_bf16(BM, H, 0, 0);
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(&b_full, (uint32_t)(2 * H * 128));
       for (int kb = 0; kb < 2; ++kb) tma_load_2d(sB + (size_t)kb * H * 128, &t_whp, &b_full, c * NG + kb * 64, 0);
     }
     for (int k = 0; k < T - 1; ++k) { cl_arrive(); cl_wait(); }
-  } else if (warp == 1) {
-    if (lane == 0) mbar_wait(&b_full, 0);
-    __syncwarp();
-    for (int k = 0; k < T - 1; ++k) {
-      if (lane == 0) {
-        mbar_wait(&a_ready, k & 1);                    // dz_s of the own units is in sA
-        tc_fence_after();
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb) {
-          const uint32_t sa = smem_u32(sA + (size_t)kb * BM * 128);
-          const uint32_t sb = smem_u32(sB + (size_t)kb * H * 128);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk)
-            mma_f16(tmem_base, make_smem_desc(sa + kk * 32, 16, 1024), make_smem_desc(sb + kk * 32, 16, 1024),
-                    idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-        }
-        mma_commit(&acc_full);
-      }
-      __syncwarp();
-      cl_arrive(); cl_wait();
-    }
   } else {
-    const int ew = warp - 2;
-    const int q = warp & 3, half = ew >> 2;
-    const int r = q * 32 + lane;
-    const int b = row0 + r;
-    const bool active = q * 32 < R;
-    const bool valid = active && b < B;
-    const int j0 = c * U + half * UH;
-    // where the partial sums of this thread's 16 units sit inside a source CTA's lane-major buffer
-    const int n0 = j0;                                // first column (unit) wanted
-    const int src_half = n0 / (H / 2);
-    const int src_v = (n0 % (H / 2)) / 8;
-    const int src_ew = src_half * 4 + ((q + 2) & 3);
-    const int cta0 = (blockIdx.x / csize) * csize;    // first CTA of this cluster
-    float dcs[UH];
+    reg_alloc<232>();
+    const int tid = threadIdx.x - 128, ew = tid >> 5, wgc = ew >> 2;
+    const bool mma = wgc < nwg;
+    const int cta0 = (blockIdx.x / CS) * CS;          // first CTA of this cluster
+    if (mma) mbar_wait(&b_full, 0);
+    float dcs[16];
 #pragma unroll
-    for (int j = 0; j < UH; ++j) dcs[j] = 0.f;
+    for (int j = 0; j < 16; ++j) dcs[j] = 0.f;
     for (int s = T - 1; s >= 0; --s) {
       const int k = T - 1 - s;
-      uint4 pk[4][2];
-      if (active) {
-        // -------- A phase: dh_s -> dz_s of the own units
-        float gi[UH], gf[UH], gg[UH], go[UH], cc[UH], cp[UH], dh[UH];
+      if (mma) {
+        // -------- dh_s -> dz_s of the own units
+        float gi[16], gf[16], gg[16], go[16], cc[16], cp[16], dh[16];
         {
           const uint4* sp = p.state + state_idx(s, n_ctas, blockIdx.x, ew, 0, lane);
           const uint4* pp = p.state + state_idx(s > 0 ? s - 1 : 0, n_ctas, blockIdx.x, ew, 8, lane);
@@ -394,28 +337,37 @@ lstm_bwd_k(const __grid_constant__ CUtensorMap t_whp, BwdP p) {
           }
         }
 #pragma unroll
-        for (int j = 0; j < UH; ++j) dh[j] = 0.f;
+        for (int j = 0; j < 16; ++j) dh[j] = 0.f;
         if (p.seq || s == T - 1) {
-          const uint4* e4 = reinterpret_cast<const uint4*>(p.err + (size_t)(valid ? b : 0) * p.lde +
-                                                           (p.seq ? (size_t)s * H : 0) + j0);
-          unpack8(e4[0], dh);
-          unpack8(e4[1], dh + 8);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int b = row0 + slot_row(ew, lane, 2 * h);
+            if (slot_row(ew, lane, 2 * h) < R && b < B) {
+              const __nv_bfloat16* e = p.err + (size_t)b * p.lde + (p.seq ? (size_t)s * H : 0) + c * U;
+#pragma unroll
+              for (int ii = 0; ii < 4; ++ii) {
+                const int j = 4 * ii + 2 * h;
+                const __nv_bfloat162 x = *reinterpret_cast<const __nv_bfloat162*>(e + slot_unit(lane, j));
+                dh[j] = __low2float(x); dh[j + 1] = __high2float(x);
+              }
+            }
+          }
         }
         if (k > 0) {
           cl_wait();                                   // phase k - 1: every CTA's partial sums are out
           const uint4* pb = p.part + (size_t)((k - 1) & 1) * part_buf;
-          for (int src = 0; src < csize; ++src) {
-            const uint4* pv = pb + ((size_t)((cta0 + src) * 8 + src_ew) * NV + src_v) * 32 + lane;
+          for (int src = 0; src < CS; ++src) {
+            const uint4* pv = pb + ((size_t)((cta0 + src) * CS + c) * 256 + tid) * 2;
             float t0[8], t1[8];
             unpack8(__ldcg(pv), t0);
-            unpack8(__ldcg(pv + 32), t1);
+            unpack8(__ldcg(pv + 1), t1);
 #pragma unroll
             for (int j = 0; j < 8; ++j) { dh[j] += t0[j]; dh[8 + j] += t1[j]; }
           }
         }
-        float zz[4][UH];
+        float zz[4][16];
 #pragma unroll
-        for (int j = 0; j < UH; ++j) {
+        for (int j = 0; j < 16; ++j) {
           const float tc = 1.7159f * tanh_fast(0.6666f * cc[j]);
           const float dtc = fmaf(tc * tc, -0.388484177f, 1.14381894f);        // d(A tanh(B c)) / dc
           const float dc = fmaf(dh[j] * go[j], dtc, dcs[j]);
@@ -425,60 +377,69 @@ lstm_bwd_k(const __grid_constant__ CUtensorMap t_whp, BwdP p) {
           zz[3][j] = dh[j] * tc * go[j] * (1.f - go[j]);
           dcs[j] = dc * gf[j];
         }
-#pragma unroll
-        for (int g = 0; g < 4; ++g) { pk[g][0] = pack8(zz[g]); pk[g][1] = pack8(zz[g] + 8); }
         if (s > 0) {
           // own A operand: k index = gate * 32 + local unit (the order W_h^T was permuted to)
 #pragma unroll
           for (int g = 0; g < 4; ++g) {
             uint8_t* blk = sA + (size_t)(g >> 1) * BM * 128;
-            const int ch = (g & 1) * 4 + half * 2;
-            *reinterpret_cast<uint4*>(blk + sw128(r, ch)) = pk[g][0];
-            *reinterpret_cast<uint4*>(blk + sw128(r, ch + 1)) = pk[g][1];
+#pragma unroll
+            for (int j = 0; j < 16; j += 2) {
+              const int r = slot_row(ew, lane, j), u = (g & 1) * 32 + slot_unit(lane, j);
+              *reinterpret_cast<__nv_bfloat162*>(blk + sw128(r, u >> 3) + (u & 7) * 2) =
+                  __floats2bfloat162_rn(zz[g][j], zz[g][j + 1]);
+            }
           }
           fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&a_ready);
         }
-        if (valid) {
-          __nv_bfloat16* dr = p.dz + ((size_t)s * B + b) * 4 * H + j0;
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            reinterpret_cast<uint4*>(dr + (size_t)g * H)[0] = pk[g][0];
-            reinterpret_cast<uint4*>(dr + (size_t)g * H)[1] = pk[g][1];
+        for (int h = 0; h < 2; ++h) {
+          const int b = row0 + slot_row(ew, lane, 2 * h);
+          if (slot_row(ew, lane, 2 * h) < R && b < B) {
+            __nv_bfloat16* dr = p.dz + ((size_t)s * B + b) * 4 * H + c * U;
+#pragma unroll
+            for (int g = 0; g < 4; ++g)
+#pragma unroll
+              for (int ii = 0; ii < 4; ++ii) {
+                const int j = 4 * ii + 2 * h;
+                *reinterpret_cast<__nv_bfloat162*>(dr + (size_t)g * H + slot_unit(lane, j)) =
+                    __floats2bfloat162_rn(zz[g][j], zz[g][j + 1]);
+              }
           }
+        }
+        if (s > 0) {
+          // -------- P = dz_s[:, own] . W_h[own, :] -> bf16 pieces for the owners of its columns
+          named_bar_sync(1 + wgc, 128);                // the warpgroup's rows of sA are complete
+          float acc[HN / 2];
+          wg_fence();
+#pragma unroll
+          for (int kb = 0; kb < 2; ++kb) {
+            const uint32_t sa = smem_u32(sA + (size_t)kb * BM * 128) + wgc * 8192;
+            const uint32_t sb = smem_u32(sB + (size_t)kb * H * 128);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+              wgmma_bf16<HN, 0, 0>(acc, make_smem_desc(sa + kk * 32, 16, 1024), make_smem_desc(sb + kk * 32, 16, 1024),
+                                   (kb > 0 || kk > 0) ? 1 : 0);
+          }
+          wg_commit();
+          wg_wait<0>();
+          wg_fence_regs(acc);
+          // owner d of columns [32 d, 32 d + 32) holds the same fragment rows: registers 16 d .. 16 d + 15
+          uint4* pw = p.part + (size_t)(k & 1) * part_buf + ((size_t)blockIdx.x * CS * 256 + tid) * 2;
+#pragma unroll
+          for (int d = 0; d < CS; ++d) {
+            pw[(size_t)d * 512] = pack8(acc + 16 * d);
+            pw[(size_t)d * 512 + 1] = pack8(acc + 16 * d + 8);
+          }
+          // sA is rewritten next step only after every thread of this warpgroup passed its MMA
+          named_bar_sync(1 + wgc, 128);
         }
       } else if (k > 0) {
         cl_wait();
       }
       if (s == 0) break;
-      // -------- B phase: P = dz_s[:, own] . W_h[own, :] -> lane-major bf16 pieces for their owners
-      if (active) {
-        mbar_wait(&acc_full, k & 1);
-        tc_fence_after();
-        uint4* pw = p.part + (size_t)(k & 1) * part_buf + ((size_t)(blockIdx.x * 8 + ew) * NV) * 32 + lane;
-        for (int v0 = 0; v0 < NV; v0 += 4) {
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * (H / 2) + v0 * 8), v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int w4 = 0; w4 < 4; ++w4) {
-            uint4 o;
-            o.x = pack_bf16(__uint_as_float(v[8 * w4]), __uint_as_float(v[8 * w4 + 1]));
-            o.y = pack_bf16(__uint_as_float(v[8 * w4 + 2]), __uint_as_float(v[8 * w4 + 3]));
-            o.z = pack_bf16(__uint_as_float(v[8 * w4 + 4]), __uint_as_float(v[8 * w4 + 5]));
-            o.w = pack_bf16(__uint_as_float(v[8 * w4 + 6]), __uint_as_float(v[8 * w4 + 7]));
-            pw[(size_t)(v0 + w4) * 32] = o;
-          }
-        }
-        tc_fence_before();
-      }
       cl_arrive();                                     // phase k: this thread's partial sums are out
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, tcols); }
 }
 
 // W_h^T in the k order of the backward kernel: dst[n][c * 128 + g * 32 + j] = w[g * H + c * 32 + j][col0 + n]
@@ -506,22 +467,24 @@ __global__ void lstm_unpack_state_k(const uint4* __restrict__ state, float* __re
     const int ew = (int)((i / (32 * SVEC)) % 8);
     const int cta = (int)((i / (32 * SVEC * 8)) % n_ctas);
     const int t = (int)(i / ((size_t)32 * SVEC * 8 * n_ctas));
-    const int q = (ew + 2) & 3, half = ew >> 2;
-    const int r = q * 32 + lane;
-    const int b = (cta / csize) * R + r;
-    if (r >= R || b >= B) continue;
-    const int j = (cta % csize) * U + half * UH;
     const uint4 val = state[i];
+    const int n = v < 8 ? 8 : 4;                      // slots in this vector
+    const int s0 = v < 8 ? 8 * (v & 1) : 4 * (v - 8);
+    float f[8];
     if (v < 8) {
-      float f[8];
       unpack8(val, f);
-      float* dst = gates + ((size_t)t * B + b) * 4 * H + (size_t)(v >> 1) * H + j + 8 * (v & 1);
-      reinterpret_cast<float4*>(dst)[0] = make_float4(f[0], f[1], f[2], f[3]);
-      reinterpret_cast<float4*>(dst)[1] = make_float4(f[4], f[5], f[6], f[7]);
     } else {
-      float* dst = cells + ((size_t)t * B + b) * H + j + 4 * (v - 8);
-      *reinterpret_cast<float4*>(dst) = make_float4(__uint_as_float(val.x), __uint_as_float(val.y),
-                                                    __uint_as_float(val.z), __uint_as_float(val.w));
+      f[0] = __uint_as_float(val.x); f[1] = __uint_as_float(val.y);
+      f[2] = __uint_as_float(val.z); f[3] = __uint_as_float(val.w);
+    }
+    for (int k = 0; k < n; ++k) {
+      const int sl = s0 + k;
+      const int r = slot_row(ew, lane, sl);
+      const int b = (cta / csize) * R + r;
+      if (r >= R || b >= B) continue;
+      const int j = (cta % csize) * U + slot_unit(lane, sl);
+      if (v < 8) gates[((size_t)t * B + b) * 4 * H + (size_t)(v >> 1) * H + j] = f[k];
+      else cells[((size_t)t * B + b) * H + j] = f[k];
     }
   }
 }
@@ -637,8 +600,9 @@ int launch_lstm_bwd_persist(const void* err, long long lde, int seq, const void*
   if (smem > 227 * 1024 - 2048) return -4;
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(lstm_bwd_k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 2048) != cudaSuccess)
-      return -5;
+    for (auto k : {lstm_bwd_k<64>, lstm_bwd_k<128>, lstm_bwd_k<192>, lstm_bwd_k<256>})
+      if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 2048) != cudaSuccess)
+        return -5;
     attr_set = true;
   }
   // W_h^T [H][4H], columns permuted to (CTA, gate, unit) order, from the bf16 weight shadow
@@ -652,7 +616,9 @@ int launch_lstm_bwd_persist(const void* err, long long lde, int seq, const void*
   const int R = lstm_persist_rows(B, H);
   BwdP p{T, B, H, R, (const __nv_bfloat16*)err, lde, seq, (const uint4*)state, (uint4*)part, (__nv_bfloat16*)dz};
   const int clusters = (B + R - 1) / R;
-  r = launch_cluster(lstm_bwd_k, clusters * csize, csize, smem, st, t_whp, p);
+  void (*kern)(const CUtensorMap, BwdP) = H == 64 ? lstm_bwd_k<64> : H == 128 ? lstm_bwd_k<128>
+                                            : H == 192 ? lstm_bwd_k<192> : lstm_bwd_k<256>;
+  r = launch_cluster(kern, clusters * csize, csize, smem, st, t_whp, p);
   if (r == 0) ++g_lstm_persist_launches;
   return r == 0 ? 0 : -7;
 }
@@ -660,7 +626,7 @@ int launch_lstm_bwd_persist(const void* err, long long lde, int seq, const void*
 void launch_lstm_unpack_state(const void* state, float* gates, float* cells, int T, int B, int H,
                               cudaStream_t st) {
   using namespace lp;
-  lstm_unpack_state_k<<<296, 256, 0, st>>>((const uint4*)state, gates, cells, T, B, H, lstm_persist_rows(B, H),
+  lstm_unpack_state_k<<<2 * num_sms(), 256, 0, st>>>((const uint4*)state, gates, cells, T, B, H, lstm_persist_rows(B, H),
                                            lstm_ctas(B, H));
 }
 

@@ -481,11 +481,9 @@ pool_backward_win_k(const T* __restrict__ err_out, const int* __restrict__ offs,
   st8(err_in + (size_t)i * 8, s);
 }
 
-// Per-kernel ncu timing on B200 (CIFAR layers, bf16): the fixed-window FORWARD kernel is faster
-// than the generic one (3.7-4.2 us vs 5.2-5.9 us, pool1 7.1 vs 7.7 us) and is the default; the
-// fixed-window BACKWARD kernel is slower (pool1 27 us vs 17.5 us: 4 positions x (err + offsets +
-// output) held in registers costs more occupancy than the serialised round trips it removes)
-// and stays opt-in (ZNICZ_POOL_WIN_BWD=1). ZNICZ_POOL_WIN=0 disables both.
+// The fixed-window FORWARD kernel is the default; the fixed-window BACKWARD kernel (4 positions x
+// (err + offsets + output) held in registers, which costs occupancy) stays opt-in
+// (ZNICZ_POOL_WIN_BWD=1). ZNICZ_POOL_WIN=0 disables both.
 static bool pool_win_enabled(bool backward) {
   static int fwd = -1, bwd = -1;
   if (fwd < 0) {

@@ -75,7 +75,7 @@ __global__ void s2d_unpack_grad_k(const float* __restrict__ gs, float* __restric
 
 static int grid_of(long long total) {
   long long b = (total + 255) / 256;
-  if (b > 148 * 32) b = 148 * 32;
+  if (b > 32LL * num_sms()) b = 32LL * num_sms();
   return (int)(b < 1 ? 1 : b);
 }
 

@@ -1,6 +1,6 @@
 // Kohonen self-organising map kernels — the reference has only OpenCL kernels for this op
 // (/root/reference/ocl/kohonen.cl:19,59,139,161,182: calculate_distances, calculate_argmin,
-// set_total, compute_gravity, apply_gradient); this is a CUDA design for sm_100a:
+// set_total, compute_gravity, apply_gradient); this is a CUDA design for sm_90a:
 //   som_winners_k : one CTA per sample, warp-shuffle argmin of ||w_n - x||^2, winners histogram
 //   som_update_k  : one thread per (neuron, feature); sums gravity * (x - w) over the batch and
 //                   applies the step (batch semantics identical to the numpy oracle)
@@ -67,7 +67,7 @@ __global__ void som_update_k(const float* __restrict__ x, float* __restrict__ w,
 // GEMM formulation (the reference's calculate_distances is its tiled matmul with a custom
 // MULTIPLY, /root/reference/ocl/kohonen.cl:19-36). ||w_n - x_s||^2 = |x_s|^2 - 2 x_s.w_n + |w_n|^2,
 // so the winners are argmin_n (|w_n|^2 - 2 x_s.w_n): one [batch x neurons x len] GEMM on the
-// tcgen05 kernel. fp32 operands are split into bf16 hi + lo parts and the three significant
+// wgmma kernel. fp32 operands are split into bf16 hi + lo parts and the three significant
 // products (hi*hi + hi*lo + lo*hi) are folded into ONE GEMM by concatenating along K:
 //   A' = [x_hi | x_hi | x_lo],  B' = [w_hi | w_lo | w_hi]   (K' = 3 * roundup(len, 8))
 // which keeps ~16 bits of every product - enough for the argmin to agree with the fp32 oracle

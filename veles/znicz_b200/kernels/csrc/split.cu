@@ -1,7 +1,7 @@
 // fp32 -> bf16 hi/lo part splitter for the "fp32 on the tensor cores" path (kernels/fp32x.py).
 //
 // x = hi + lo with hi = bf16(x), lo = bf16(x - hi) carries 16 mantissa bits; the product of two
-// split operands  x.w ~= hi.hi + hi.lo + lo.hi (+ lo.lo)  is evaluated by ONE bf16 tcgen05 GEMM whose
+// split operands  x.w ~= hi.hi + hi.lo + lo.hi (+ lo.lo)  is evaluated by ONE bf16 wgmma GEMM whose
 // reduction dimension holds the parts side by side:
 //     A side, pattern 0: [hi | hi | lo | lo]      B side, pattern 1: [hi | lo | hi | lo]
 // (3 parts drop the lo.lo term: 2^-18 relative). The fp32 accumulator of the tensor core adds the
@@ -77,7 +77,7 @@ void launch_split_parts(const float* src, long long rows, int len, __nv_bfloat16
   const int kmax = (b && b_kp > a_kp) ? b_kp : a_kp;
   const long long total = rows * kmax;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 16LL * num_sms()) blocks = 16LL * num_sms();
   if (blocks < 1) blocks = 1;
   launch_k(split_parts_k, (int)blocks, 256, 0, st, src, rows, len, kmax, da, db);
 }
@@ -86,7 +86,7 @@ void launch_split_conv_wt(const float* w, __nv_bfloat16* dst, int F, int taps, i
                           int nparts, int pattern, cudaStream_t st) {
   const long long total = (long long)taps * Fp * Cp;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 16LL * num_sms()) blocks = 16LL * num_sms();
   launch_k(split_conv_wt_k, (int)blocks, 256, 0, st, w, dst, F, taps, C, Fp, Cp, nparts, pattern);
 }
 

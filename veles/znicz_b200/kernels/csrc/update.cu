@@ -11,10 +11,10 @@
 //   acc  = acc_beta * acc + acc_alpha * gd ; gd = gd_beta * gd + gd_alpha * acc      (optional)
 //   gd  += moment * vel ; vel = gd                                                     (optional)
 //   w   += gd                                                                          (optional)
-//   + bf16 shadow copies of w in the layouts the tcgen05 GEMM/conv kernels consume.
+//   + bf16 shadow copies of w in the layouts the wgmma GEMM/conv kernels consume.
 //
 // In data-parallel mode grad[r] are *peer pointers* into the other GPUs' HBM (symmetric
-// memory over NVLink5/NVSwitch): every rank reads all ranks' gradient tiles in the same order,
+// memory over NVLink/NVSwitch): every rank reads all ranks' gradient tiles in the same order,
 // so all replicas compute bit-identical weights with no NCCL call and no broadcast.
 // Cross-GPU ordering uses per-block flag words in symmetric memory (st.release.sys /
 // ld.acquire.sys), with the epoch counter kept in device memory so CUDA-graph replays work.
@@ -800,7 +800,8 @@ void launch_multi_update(const void* table, int n, int total_tiles, int has_orth
   if (peer_flags) for (int r = 0; r < nranks; ++r) ps.flags[r] = peer_flags[r];
   GridSync gs{gridsync, gridsync + 1};
   // latency-bound kernel: 4 CTAs of 256 threads per SM (all co-resident: the grid barrier needs it)
-  int blocks = total_tiles < 592 ? total_tiles : 592;
+  const int resident = 4 * num_sms();
+  int blocks = total_tiles < resident ? total_tiles : resident;
   if (ps.nranks > 1 && blocks > MU_MAX_PEER_BLOCKS) blocks = MU_MAX_PEER_BLOCKS;
   if (blocks < 1) blocks = 1;
   RedBufs rb{};
@@ -817,7 +818,7 @@ void launch_multi_update(const void* table, int n, int total_tiles, int has_orth
 int fused_update_blocks(long long size) {
   long long b = (size + 255) / 256;     // one element per thread up to one CTA per SM
   if (b < 1) b = 1;
-  if (b > 148) b = 148;
+  if (b > num_sms()) b = num_sms();
   return (int)b;
 }
 
@@ -852,7 +853,7 @@ void launch_refresh_shadows(const float* w, long long size, int rows, int cols, 
                             __nv_bfloat16* lp_conv, int taps, int C, int c_pad, int lp_cpad,
                             cudaStream_t st) {
   ShadowSpec sh{lp, ld, lp_cpad, lp_conv, taps, C, c_pad};
-  long long b = (size + 255) / 256; if (b > 592) b = 592; if (b < 1) b = 1;
+  long long b = (size + 255) / 256; if (b > 4 * num_sms()) b = 4 * num_sms(); if (b < 1) b = 1;
   launch_k(refresh_shadows_k, (int)b, 256, 0, st, w, size, rows, cols, sh);
 }
 

@@ -1,14 +1,14 @@
-"""fp32 layers on the tcgen05 tensor cores ("split-bf16", SURVEY §6 config 2).
+"""fp32 layers on the wgmma tensor cores ("split-bf16", SURVEY §6 config 2).
 
 ``compute_type: "fp32"`` keeps activations, errors and weights in fp32 - the reference's only
 precision (/root/reference/all2all.py:262-275 calls SGEMM, conv.py:330-352 its fp32 im2col GEMM).
-The 5th-generation tensor cores have no fp32 operand type, so each fp32 operand is written as
+The tensor cores have no fp32 operand type, so each fp32 operand is written as
 ``hi + lo`` (two bf16 numbers = 16 mantissa bits, kernels/csrc/split.cu) and the product
 
     x . w  ~=  hi.hi + hi.lo + lo.hi (+ lo.lo)
 
-is evaluated by ONE bf16 tcgen05 GEMM / implicit-GEMM convolution whose reduction dimension holds
-the parts side by side; the fp32 TMEM accumulator sums the partial products. The same kernels as
+is evaluated by ONE bf16 wgmma GEMM / implicit-GEMM convolution whose reduction dimension holds
+the parts side by side; the fp32 accumulator sums the partial products. The same kernels as
 the bf16 path run (gemm_umma.cu: TMA, tap-mode im2col gather, split-K), on 3-4x the reduction
 length - still several times faster than the SIMT fp32 kernels, at ~1e-5 relative error per
 product instead of bf16's 4e-3.

@@ -145,7 +145,7 @@ def apply_config_file(path):
 def build_parser():
     p = argparse.ArgumentParser(
         prog="python -m veles.znicz_b200",
-        description="Run a Znicz workflow on B200 (or the numpy backend).")
+        description="Run a Znicz workflow on H100 (or the numpy backend).")
     p.add_argument("workflow", help="workflow .py file, dotted module or sample name "
                                     "(wine, mnist, cifar, ...)")
     p.add_argument("config", nargs="?", default=None,

@@ -11,7 +11,7 @@ when there is no validation set) and ``epoch_number`` advances when TRAIN wraps.
 The last minibatch of a class may be short: buffers are max-sized, the tail is
 zero-filled (labels -1) and ``minibatch_size`` carries the real count.
 
-B200 path: the minibatch is staged in pinned host memory and copied H2D on a
+H100 path: the minibatch is staged in pinned host memory and copied H2D on a
 dedicated copy stream into one of two device buffers (double buffering, the
 ``Avatar`` equivalent), together with a small device-side header
 ``[minibatch_size, minibatch_class]`` so captured CUDA graphs read the runtime
@@ -355,7 +355,7 @@ class Loader(AcceleratedUnit, metaclass=UserLoaderRegistry):
                     self.epoch_number >= self.epoch_limit):
                 self.complete <<= True
 
-    # -- B200 staging -----------------------------------------------------------------
+    # -- H100 staging -----------------------------------------------------------------
     def _staged_arrays(self):
         """Arrays copied H2D every step."""
         arrs = [self.minibatch_data]

@@ -8,8 +8,8 @@ Data layout: ``original_data[total, ...]`` ordered TEST, VALID, TRAIN;
 ``original_labels`` a python list / int32 array of raw labels mapped to
 0..n-1 via ``labels_mapping``.
 
-B200: with ``on_device=True`` (default when the dataset fits comfortably — 180 GB
-of HBM3e makes that the common case) the dataset is uploaded once and every
+H100: with ``on_device=True`` (default when the dataset fits comfortably in the
+80 GB of HBM3) the dataset is uploaded once and every
 minibatch is produced by a device gather kernel (``gather_rows``), so no host
 traffic happens in the training loop; with ``on_device=False`` minibatches are
 staged through pinned memory each step (streaming mode, the path ``bench.py``
@@ -380,7 +380,7 @@ class FullBatchLoader(Loader, LoaderWithValidationRatio):
         hn[2] = self.epoch_number
         hn[4:4 + self.max_minibatch_size] = self.minibatch_indices.mem
         if _pull_ok(self.device.ext):
-            # no copy-engine operation in the step's stream (profiles/host_vs_device_r1.md)
+            # no copy-engine operation in the step's stream
             self.device.ext.pull_from_host(pd["hdr_idx"][slot], self._hdr_idx_dev_)
         else:
             self._hdr_idx_dev_.copy_(pd["hdr_idx"][slot], non_blocking=True)

@@ -9,7 +9,7 @@ Dataset files (produced by ``utils/preparation_imagenet.py``):
   ``count_samples_filename``    json {"test": n, "val": n, "train": n}
   ``matrixes_filename``         pickle [mean (sy, sx, c) uint8/float, rdisp (sy, sx, c)]
 
-B200 notes: the sample file is memory-mapped; a minibatch is gathered with one fancy-index
+H100 notes: the sample file is memory-mapped; a minibatch is gathered with one fancy-index
 read into the pinned staging buffer (no per-sample ``seek``/``readinto`` loop), cropping and
 mirroring are vectorised over the minibatch, and ``mean``/``rdisp`` are exported for the
 device-side ``MeanDispNormalizer`` unit exactly like the reference.

@@ -3,7 +3,7 @@
 Each class has a random smooth prototype; samples are prototype + noise, so the
 nets actually learn (convergence tests) while shapes/dtypes match the reference
 configs: MNIST 28×28×1 / 10 classes, CIFAR-10 32×32×3 / 10, ImageNet-style
-227×227×3 / 1000 (bench shapes from BASELINE.json).
+227×227×3 / 1000 (the bench.py shapes).
 """
 from __future__ import annotations
 

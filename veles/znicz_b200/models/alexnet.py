@@ -7,7 +7,7 @@ imagenet_workflow_config.py:94-250, imagenet_workflow_nin_config.py,
 imagenet_workflow_vgga_config.py, and the LMDB variant imagenet_workflow_lmdb_config.py.
 The layer lists are generated from compact tables instead of being spelled out.
 
-B200: on the CUDA backend all conv/FC layers run on the tcgen05 implicit-GEMM kernels in
+H100: on the CUDA backend all conv/FC layers run on the wgmma implicit-GEMM kernels in
 bf16 with fp32 accumulation; FC6 (9216x4096) is the tensor the two-shot fused reduce+update
 exists for in data-parallel runs.
 """

@@ -3,7 +3,7 @@
 Parity: /root/reference/samples/DemoKohonen/kohonen.py:50-154, kohonen_config.py:40-60
 (KohonenTrainer + KohonenDecision, 200 epochs, decay lambdas in the config, three SOM
 plotters and a Shell unit in the loop). The reference forces the OpenCL backend
-(kohonen_config.py:40); here the trainer runs on the B200 kernels (``csrc/som.cu``) or numpy.
+(kohonen_config.py:40); here the trainer runs on the H100 kernels (``csrc/som.cu``) or numpy.
 """
 from __future__ import annotations
 

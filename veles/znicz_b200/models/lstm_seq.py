@@ -4,7 +4,7 @@
 The reference builds sequences by chaining single-step ``LSTM`` sub-workflows and sharing their
 weights (/root/reference/lstm.py:52-143, BPTT through ``GDLSTM.err_prev_output/err_prev_memory``
 :263,304); here the ``lstm_seq`` layer (ops/lstm_seq.py) runs all time steps of a minibatch
-[batch][T][features] inside one unit - one tcgen05 GEMM + one fused cell kernel per step, a single
+[batch][T][features] inside one unit - one wgmma GEMM + one fused cell kernel per step, a single
 weight-gradient GEMM over the whole sequence - followed by a softmax classifier on the last
 hidden state.
 """

@@ -62,7 +62,7 @@ class NativeEngine(object):
 
     @property
     def tensor_core_launches(self):
-        """tcgen05 GEMM / conv launches issued by the CUDA executor so far."""
+        """wgmma GEMM / conv launches issued by the CUDA executor so far."""
         return int(self._lib.znicz_engine_tc_launches(self._h))
 
     @staticmethod

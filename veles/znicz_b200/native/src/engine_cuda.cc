@@ -1,8 +1,8 @@
-// sm_100a executor of the native runtime: launches the training engine's own kernels through
+// sm_90a executor of the native runtime: launches the training engine's own kernels through
 // their C++ launchers - no libtorch, no cuBLAS. Weights are uploaded once and stay resident in HBM.
-// FC and conv layers run on the tcgen05 tensor cores with fp32-class accuracy: weights are split
+// FC and conv layers run on the wgmma tensor cores with fp32-class accuracy: weights are split
 // ONCE at load time into bf16 hi/lo parts laid side by side along the reduction dimension, the
-// activations per call (csrc/split.cu), one bf16 tcgen05 GEMM / implicit-GEMM conv
+// activations per call (csrc/split.cu), one bf16 wgmma GEMM / implicit-GEMM conv
 // (csrc/gemm_umma.cu) accumulates hi.hi + hi.lo + lo.hi (+ lo.lo) in fp32 - the scheme of
 // kernels/fp32x.py. ZNICZ_NATIVE_TC=0 (or a shape the kernels decline) keeps the SIMT fp32 kernels
 // (csrc/gemm_simt.cu); pooling / LRN / activations / softmax are the training kernels as well.

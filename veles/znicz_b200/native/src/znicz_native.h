@@ -1,11 +1,11 @@
 // znicz_native — forward-only inference runtime for packages written by
 // veles.znicz_b200.export.package (contents.json + NNNN_shape.npy in a zip).
 //
-// B200-native equivalent of the reference's libZnicz (/root/reference/libZnicz: All2All,
+// H100-native equivalent of the reference's libZnicz (All2All,
 // All2AllLinear/Tanh/Softmax on libVeles+libSimd, single sample, CPU/NEON), extended to every
 // exportable forward unit (conv, pooling, LRN, activations, cutter, dropout) and to batches.
 // Two executors over one unit list: a portable CPU executor (the oracle of the C++ tests) and
-// an sm_100a executor that launches the same hand-written kernels as the training engine
+// an sm_90a executor that launches the same hand-written kernels as the training engine
 // (no libtorch, no cuBLAS/cuDNN).
 #pragma once
 #include <cstdint>
@@ -74,10 +74,10 @@ class Engine {
   Shape4 infer(const Shape4& in);
   // CPU executor. input: n*h*w*c floats. Returns the last unit's output.
   std::vector<float> run_cpu(const float* input, const Shape4& in);
-  // sm_100a executor (throws std::runtime_error when no CUDA device is usable).
+  // sm_90a executor (throws std::runtime_error when no CUDA device is usable).
   std::vector<float> run_cuda(const float* input, const Shape4& in);
   static bool cuda_available();
-  // tcgen05 GEMM / conv launches issued by run_cuda() so far (0: every layer took the SIMT path)
+  // wgmma GEMM / conv launches issued by run_cuda() so far (0: every layer took the SIMT path)
   long long cuda_tensor_core_launches() const;
 
  private:

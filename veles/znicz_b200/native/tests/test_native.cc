@@ -1,6 +1,6 @@
 // C++ tests of the native runtime (mirrors /root/reference/libZnicz/tests/all2all*.cc:
 // typed fixtures with hand-computed expectations to 1e-6 relative), plus package parsing,
-// conv/pool/LRN/cutter units and (when a GPU is present) CPU-vs-sm_100a agreement.
+// conv/pool/LRN/cutter units and (when a GPU is present) CPU-vs-sm_90a agreement.
 #include "../src/znicz_native.h"
 
 #include <cmath>

@@ -7,7 +7,7 @@ TanhLog :525/553, SinCos :589/609). Reference bugs are *not* reproduced: sigmoid
 the documented 1/(1+e^-x) (the CUDA kernel computes e^x, cuda/activation.cu:32),
 StrictRELU selects from the input, Log/TanhLog work on the device.
 
-B200: one vectorised elementwise kernel family (``act_forward`` / ``act_backward``,
+H100: one vectorised elementwise kernel family (``act_forward`` / ``act_backward``,
 16-byte accesses, bf16 or fp32 storage, fp32 math). In StandardWorkflow graphs the
 activation that directly follows a conv/FC is normally folded into that GEMM's
 epilogue; these units exist for the composable API.

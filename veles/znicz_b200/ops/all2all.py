@@ -6,8 +6,8 @@ Weight init magnitude ``min(sqrt(C/(in+out)), 0.5)`` (:106-117,154-155); fill mo
 uniform/gaussian/constant; FC weights are ``[neurons, input_size]`` and
 ``weights_transposed`` flips the storage to ``[input_size, neurons]``.
 
-B200 path: one tcgen05 GEMM whose epilogue applies bias + activation while the
-accumulator tile is read out of TMEM (``gemm_bias_act``); softmax adds a row
+H100 path: one wgmma GEMM whose epilogue applies bias + activation to the
+register accumulator tile (``gemm_bias_act``); softmax adds a row
 kernel that also records ``max_idx``. No cuBLAS on this path.
 """
 from __future__ import annotations
@@ -100,7 +100,7 @@ class All2All(nn_units.FullyConnectedOutput, nn_units.NNLayerBase):
         self.numpy_linear()
         apply_activation_numpy(self.output.mem, self.ACT)
 
-    # -- sm_100a ------------------------------------------------------------------------
+    # -- sm_90a ------------------------------------------------------------------------
     def refresh_shadows(self):
         from ..kernels import api
         api.refresh_weight_shadows(self)

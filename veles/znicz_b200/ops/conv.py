@@ -6,11 +6,11 @@ ConvSigmoid :500, ConvRELU :522 (softplus), ConvStrictRELU :547).
 ``1 + (S − K + pad) // slide`` (:161-166); weights ``[n_kernels, ky·kx·C]`` row-major
 with (ky, kx, C) order; default magnitude ``min(1/(max·sqrt(ky·kx·C)), 0.05)``.
 
-B200 path: no im2col buffer exists. ``conv_fprop`` is an implicit-GEMM tcgen05
+H100 path: no im2col buffer exists. ``conv_fprop`` is an implicit-GEMM wgmma
 kernel: producer warps gather the NHWC patches straight into 128B-swizzled shared
-memory (zero fill for the padding), one thread issues ``tcgen05.mma`` into a TMEM
-accumulator and the epilogue adds bias and applies the activation while draining
-TMEM (reference: 16-image ``Unpack1D`` + cuBLAS + a bias/activation kernel,
+memory (zero fill for the padding), one warpgroup issues ``wgmma.mma_async`` into
+register accumulators and the epilogue adds bias and applies the activation
+(reference: 16-image ``Unpack1D`` + cuBLAS + a bias/activation kernel,
 /root/reference/conv.py:268-297).
 """
 from __future__ import annotations
@@ -100,7 +100,7 @@ class Conv(ConvolutionalBase, nn_units.NNLayerBase):
         self.activation_mode = "ACTIVATION_LINEAR"
         self.exports.extend(("activation_mode", "kx", "ky", "n_kernels",
                              "padding", "sliding"))
-        self.unpack_size = kwargs.get("unpack_size", 16)  # API parity; unused on B200
+        self.unpack_size = kwargs.get("unpack_size", 16)  # API parity; unused on H100
         self.weights_shape = None
 
     def get_weights_magnitude(self):
@@ -224,7 +224,7 @@ class Conv(ConvolutionalBase, nn_units.NNLayerBase):
         apply_activation_numpy(out, self.ACT)
         self.output.mem[...] = out.reshape(self.output.shape)
 
-    # -- sm_100a ------------------------------------------------------------------------
+    # -- sm_90a ------------------------------------------------------------------------
     def refresh_shadows(self):
         from ..kernels import api
         api.refresh_weight_shadows(self)

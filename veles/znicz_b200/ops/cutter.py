@@ -3,7 +3,7 @@
 Parity: /root/reference/cutter.py (Cutter :91, GDCutter :177, Cutter1D :263):
 ``padding=(left, top, right, bottom)`` is what gets cut *off*; backward = zero fill +
 paste; ``Cutter1D``: ``y[:, o:o+L] = α·x[:, i:i+L] + β·y[:, o:o+L]`` (LSTM backward).
-On B200 these are single strided-copy kernels (``crop_nhwc`` / ``axpby_2d``).
+On H100 these are single strided-copy kernels (``crop_nhwc`` / ``axpby_2d``).
 """
 from __future__ import annotations
 

@@ -10,7 +10,7 @@ numpy path (:347-348); the oracle here is ``col2im(input · W)`` scaled by the o
 counts it with ``atomicAdd`` every run, /root/reference/cuda/conv/gradient_descent/
 err_input_update.cu:31, cuda/deconv/forward.cu:12).
 
-B200: the transposed conv *is* the conv dgrad gather kernel (no atomics), with the
+H100: the transposed conv *is* the conv dgrad gather kernel (no atomics), with the
 overlap scaling folded into ``alpha`` (safe) or applied as a reciprocal-hits multiply.
 """
 from __future__ import annotations

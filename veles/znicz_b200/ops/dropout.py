@@ -4,7 +4,7 @@ Parity: /root/reference/dropout.py (Dropout :55, DropoutForward :84, DropoutBack
 :191, DropoutFixer :250): active only when ``minibatch_class == TRAIN`` and not in
 ``forward_mode``; mask ∈ {0, 1/(1−p)}; evaluation = device copy (:179-187).
 
-B200: the mask comes from a counter-based hash of (seed, step, element) computed
+H100: the mask comes from a counter-based hash of (seed, step, element) computed
 in-kernel — no ``uint32[4n]`` xorshift state array (/root/reference/dropout.py:110-113);
 the numpy path uses the same hash so both paths agree bit-for-bit.
 """

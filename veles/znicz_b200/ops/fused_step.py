@@ -4,7 +4,7 @@ The reference launches one weights_update + one bias_update kernel per layer
 (/root/reference/nn_units.py:560-642, cuda/gradient_descent_common.cu) and, when
 distributed, ships every layer's weights through the master
 (/root/reference/nn_units.py:644-694). Here every GD unit only *produces* its local
-gradient (split-K partials of the tcgen05 wgrad kernels, column-sum partials for the
+gradient (split-K partials of the wgmma wgrad kernels, column-sum partials for the
 bias); a ``FusedStep`` attached to the workflow collects the parameter tensors into a
 descriptor table in HBM and, right after the last GD unit of the backward chain, launches
 ``csrc/update.cu::multi_update_k`` once: cross-GPU reduction over NVLink peer pointers +

@@ -8,8 +8,8 @@ Extra numpy-only solvers of the reference (adagrad / adadelta / fast, :111,395-4
 are provided with the *intended* maths (SURVEY §9: the reference's adagrad
 multiplies where it should divide).
 
-B200 path (kernels/api.py): act-derivative is fused into the producer of the
-two tcgen05 GEMMs' operand (one elementwise pass that also emits the column sums
+H100 path (kernels/api.py): act-derivative is fused into the producer of the
+two wgmma GEMMs' operand (one elementwise pass that also emits the column sums
 = bias gradient), dgrad and wgrad GEMMs run on tensor cores, and weights+bias
 are stepped by one fused update kernel (which is also the cross-GPU reduce).
 """
@@ -212,7 +212,7 @@ class GradientDescent(GDCommon):
         if self.on_cuda_forward_shadow():
             self.forward_unit.refresh_shadows()
 
-    # -- sm_100a ------------------------------------------------------------------------
+    # -- sm_90a ------------------------------------------------------------------------
     def cuda_run(self):
         from ..kernels import api
         api.fc_backward(self)

@@ -5,7 +5,7 @@ GDSigmoidConv :675, GDRELUConv :701, GDStrictRELUConv :726): dgrad
 (``err_input``), wgrad (``gradient_weights``), bias gradient = Σ over batch·pixels,
 then the shared fused SGD step.
 
-B200 path: dgrad is a *gather* implicit GEMM over the transposed filters (no
+H100 path: dgrad is a *gather* implicit GEMM over the transposed filters (no
 ``atomicAdd`` col2im scatter → deterministic), wgrad is a split-K implicit GEMM
 over batch·pixels whose per-CTA partials are summed in fixed order by the fused
 update kernel (reference: per-16-image Unpack1D + cuBLAS β=1 accumulation and an
@@ -118,7 +118,7 @@ class GradientDescentConv(ConvolutionalBase, GDCommon):
         if self.on_cuda_forward_shadow():
             self.forward_unit.refresh_shadows()
 
-    # -- sm_100a ------------------------------------------------------------------------
+    # -- sm_90a ------------------------------------------------------------------------
     def cuda_run(self):
         from ..kernels import api
         api.conv_backward(self)

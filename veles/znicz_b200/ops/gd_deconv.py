@@ -5,7 +5,7 @@ overlap; ``err_input = im2col(err_output) · Wᵀ``; ``gradW += inputᵀ · im2c
 shared fused weights update; no bias). numpy oracle written fresh (reference :408-409 has
 none).
 
-B200: err_input is the conv *fprop* kernel applied to the scaled err_output, wgrad is the
+H100: err_input is the conv *fprop* kernel applied to the scaled err_output, wgrad is the
 conv wgrad kernel with (image = scaled err_output, errors = deconv input).
 """
 from __future__ import annotations

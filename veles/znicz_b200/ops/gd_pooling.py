@@ -4,7 +4,7 @@ Parity: /root/reference/gd_pooling.py (GDPooling :58, GDMaxPooling :182 — also
 stochastic and pool-depool :197-198, GDMaxAbsPooling :249, GDAvgPooling :255).
 The reference has no numpy oracle for the base (:171-172); ours are vectorised.
 
-B200: the scatter kernels skip the reference's separate memset when windows do not
+H100: the scatter kernels skip the reference's separate memset when windows do not
 overlap (every input element is written exactly once by a gather formulation) and
 only fall back to zero-fill + atomics for overlapping windows.
 """

@@ -122,7 +122,7 @@ def _som_tmp(unit, name, shape, dtype):
 
 def som_winners_device(unit, x, w, argmins, winners):
     """Winners of a minibatch. Feature vectors of >= 16 elements on >= 32 neurons: distances as
-    ONE tcgen05 GEMM over bf16 hi/lo split operands (csrc/som.cu), otherwise the scalar kernel.
+    ONE wgmma GEMM over bf16 hi/lo split operands (csrc/som.cu), otherwise the scalar kernel.
     Returns the split x operand (reused by the update) or None when the scalar path ran."""
     import torch
     ext = unit.ext_
@@ -141,14 +141,14 @@ def som_winners_device(unit, x, w, argmins, winners):
     r = ext.gemm(xa, 3 * kp, False, wb, 3 * kp, True, dots, neurons, False, batch, neurons, 3 * kp,
                  None, 0, 1.0, 0.0, 1, 0, 1)
     if r != 0:
-        raise RuntimeError("%s: tcgen05 SOM distance GEMM refused (code %d)" % (unit, r))
+        raise RuntimeError("%s: wgmma SOM distance GEMM refused (code %d)" % (unit, r))
     ext.som_argmin(dots, wn, argmins, winners)
     return xa
 
 
 def som_update_device(unit, x, w, sigma, gmult):
     """w += gmult * (G . x - rowsum(G) o w) with the [neurons x len x batch] product on the
-    tcgen05 GEMM (split operands: G parts along K, x parts stacked along its rows)."""
+    wgmma GEMM (split operands: G parts along K, x parts stacked along its rows)."""
     import torch
     ext = unit.ext_
     batch, length = int(x.shape[0]), int(x.shape[1])
@@ -164,7 +164,7 @@ def som_update_device(unit, x, w, sigma, gmult):
     r = ext.gemm(ga, 3 * bp, False, xs, lp, False, m, length, False, neurons, length, 3 * bp,
                  None, 0, 1.0, 0.0, 1, 0, 1)
     if r != 0:
-        raise RuntimeError("%s: tcgen05 SOM update GEMM refused (code %d)" % (unit, r))
+        raise RuntimeError("%s: wgmma SOM update GEMM refused (code %d)" % (unit, r))
     ext.som_apply(w, m, rs, gmult)
 
 

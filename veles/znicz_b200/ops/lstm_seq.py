@@ -7,7 +7,7 @@ Here the same cell (sigmoid gates, scaled-tanh memory maker and output activatio
 peephole = the reference's ``simple`` variant) runs over ``[batch, T, features]`` inside one
 unit:
 
-  forward   per step t: z_t = [x_t | h_{t-1}] · Wᵀ + b  (one GEMM, tcgen05 in bf16 mode) and one
+  forward   per step t: z_t = [x_t | h_{t-1}] · Wᵀ + b  (one GEMM, wgmma in bf16 mode) and one
             fused cell kernel (gates, c_t, h_t; h_t is written straight into the output
             sequence and into the [x | h] operand of step t + 1);
   backward  per step (reverse): one fused cell-gradient kernel and one GEMM dz_t · W that yields

@@ -3,7 +3,7 @@
 Capability parity with /root/reference/nn_units.py (Forward :119, NNLayerBase :214,
 FullyConnectedOutput :248, GradientDescentWithActivation :299,
 GradientDescentBase :339-724, NNWorkflow :727, NNSnapshotter* :808-854), written
-fresh for the B200 engine:
+fresh for the H100 engine:
 
 * the SGD step (L1/L2 mix, orthogonality term, gradient accumulation, momentum,
   apply) is ONE fused kernel for weights and one for bias on the device

@@ -5,7 +5,7 @@ Parity: /root/reference/normalization.py (LocalResponseNormalizer :49 with
 LRNormalizerBackward :184): ``y_i = x_i · (k + α·Σ_{j∈win(i)} x_j²)^(−β)`` and the
 exact Jacobian-vector product (:224-261).
 
-B200: a warp handles pixels with the channel vector held in registers (NHWC ⇒
+H100: a warp handles pixels with the channel vector held in registers (NHWC ⇒
 one coalesced 16-byte load per 8 channels); forward/backward are one pass each.
 """
 from __future__ import annotations

@@ -11,7 +11,7 @@ StochasticPoolingDepooling :485, StochasticAbsPoolingDepooling :508, AvgPooling 
   window sum is 0 a uniformly random index is taken; randoms are 16-bit;
 * avg pooling divides by the *clipped* window size.
 
-B200: one thread handles 8 channels of one output pixel (NHWC ⇒ channels contiguous,
+H100: one thread handles 8 channels of one output pixel (NHWC ⇒ channels contiguous,
 16-byte loads); randomness is a counter-based hash of (seed, step, element) computed
 in-kernel, reproduced bit-exactly by the numpy oracle below (no state arrays, unlike
 the reference's xorshift128+ buffers).

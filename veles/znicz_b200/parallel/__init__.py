@@ -1,2 +1,2 @@
-"""Data-parallel execution on one 8×B200 node (one process per GPU)."""
+"""Data-parallel execution on one 8×H100 node (one process per GPU)."""
 from .data_parallel import DataParallel  # noqa

@@ -2,7 +2,7 @@
 
 Each GD unit's fp32 gradient staging buffers (split-K wgrad partials, bias column-sum
 partials) are allocated in CUDA symmetric memory (``torch.distributed._symmetric_memory``:
-VMM allocations exported to every rank of the node and mapped over NVLink5/NVSwitch). The
+VMM allocations exported to every rank of the node and mapped over NVLink/NVSwitch). The
 rendezvous is only *plumbing* — handle exchange — the data path is our own kernel
 (``csrc/update.cu::fused_update_k<true>``), which reads every rank's gradient tile through
 the peer pointers, reduces in fixed rank order, applies the SGD step and synchronises with

@@ -1,9 +1,10 @@
 """Block-scaled fp8 (MX format: e4m3 elements, one UE8M0 power-of-two scale per 32 consecutive
 elements of the reduction dimension) - the numerics reference of north-star config 4.
 
-`tcgen05.mma kind::mxf8f6f4` multiplies e4m3 operands whose 32-element K-blocks carry an 8-bit
-exponent scale each. The device path for it is NOT built in this tree (DESIGN.md §9); this module
-is its host-side oracle and an EMULATION switch for the numpy backend:
+Block-scaled tensor-core MMAs multiply e4m3 operands whose 32-element K-blocks carry an 8-bit
+exponent scale each; the H100 has no such instruction (its e4m3 GEMM here uses one per-tensor
+scale) and this tree builds no device path for the format. This module is its host-side oracle
+and an EMULATION switch for the numpy backend:
 
 * ``quantize`` / ``dequantize`` / ``fake_quant`` implement the format exactly (round-to-nearest-even
   to e4m3 via torch's float8 type, saturation at +-448, scale = 2^ceil(log2(amax / 448)));

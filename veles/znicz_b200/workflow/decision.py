@@ -5,7 +5,7 @@ TrivialDecision :295, DecisionGD :334-584, DecisionMSE :587-768). Reference quir
 listed in SURVEY §9 are implemented as intended (statistics really reset, the
 ``[[None]*3]*3`` aliasing removed, no pdb drop at epoch 0).
 
-Data-parallel B200: per-rank metric accumulators are summed / max-ed / min-ed across
+Data-parallel H100: per-rank metric accumulators are summed / max-ed / min-ed across
 ranks right before the epoch logic runs (``dp.reduce_metrics``), the equivalent of the
 reference's slave→master metric messages (:511-541,716-738).
 """

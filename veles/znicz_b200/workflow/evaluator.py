@@ -9,7 +9,7 @@ zeroed; labels < 0 are ignored; accumulates ``n_err[2]`` (errors, evaluated),
 MSE: ``err = (y − t) · (1/batch if mean)``, per-sample (R)MSE on *denormalised*
 values, ``metrics = [sum, max, min]``, optional nearest-``class_targets`` accuracy.
 
-B200: both are multi-CTA kernels with warp-reduced metrics and atomics into the
+H100: both are multi-CTA kernels with warp-reduced metrics and atomics into the
 small accumulators (the reference runs a single CTA and fills the confusion matrix
 serially on thread 0, /root/reference/cuda/evaluator.jcu:82-88). The runtime
 batch size and multiplier are read from a device scalar so the kernel can sit in

@@ -2,7 +2,7 @@
 
 The reference configs spell activations as separate layers (``conv`` → ``activation_str``,
 ``max_pooling`` → ``activation_str`` in cifar_caffe_config.py:86-144); the reference then
-runs one elementwise kernel per activation in each direction. On B200 these kernels are
+runs one elementwise kernel per activation in each direction. On H100 these kernels are
 pure HBM round trips, so before the units are initialised this pass folds every
 *stand-alone* tanh / softplus / strict-ReLU / sigmoid activation into its producer:
 
@@ -18,7 +18,7 @@ input and output loses nothing.
 
 A second pass (:func:`fuse_backward_derivatives`) moves the ``err_output *= f'(y)`` multiply of a
 convolutional layer into the backward kernel of the pooling layer above it (which writes that
-very ``err_output`` and has y as its own input), and lets the tcgen05 weight-gradient kernel
+very ``err_output`` and has y as its own input), and lets the wgmma weight-gradient kernel
 deliver the bias gradient as an extra product row: the conv layer's separate pass over
 ``err_output`` (one launch per layer per step in the reference, gd_conv.py:645-750) disappears. The unit graph, the layer DSL, snapshots and
 ``package_export`` are unchanged — only launches disappear. ``root.common.engine.

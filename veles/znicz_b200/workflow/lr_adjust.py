@@ -3,7 +3,7 @@
 Parity: /root/reference/lr_adjust.py (LearningRateAdjust :61, policies ``exp`` :183,
 ``fixed`` :201, ``step_exp`` :217, ``inv`` :236, ``arbitrary_step`` :252). The unit
 rewrites ``learning_rate(_bias)`` of every registered GD unit each minibatch; on
-B200 the GD units mirror those scalars into a device vector (``sync_hyper``), so
+H100 the GD units mirror those scalars into a device vector (``sync_hyper``), so
 captured CUDA graphs keep replaying while the schedule moves.
 """
 from __future__ import annotations

@@ -11,7 +11,7 @@ Parity: /root/reference/standard_workflow.py (StandardWorkflow :81, ``create_wor
 The loop is ``Repeater → Loader → forwards → Evaluator → Decision → Snapshotter →
 GDs → Repeater`` with ``EndPoint`` gated on ``~decision.complete``.
 
-B200 additions: after ``initialize`` on a CUDA device the forward chain (+evaluator)
+H100 additions: after ``initialize`` on a CUDA device the forward chain (+evaluator)
 and the GD chain are wrapped into two :class:`GraphSegment` s — the python unit graph
 still decides *what* runs each minibatch, a captured CUDA graph removes the per-unit
 launch overhead — and, when launched under ``torchrun``, a
@@ -574,7 +574,7 @@ class StandardWorkflow(StandardWorkflowBase):
             return self.gds
         raise ValueError("weights_input should be 'weights' or 'gradient_weights'")
 
-    # -- B200: CUDA-graph segments + data parallel -------------------------------------------------
+    # -- H100: CUDA-graph segments + data parallel -------------------------------------------------
     def initialize(self, device=None, **kwargs):
         if device is None or isinstance(device, str):
             from ..core.backends import get_device
