@@ -137,7 +137,7 @@ def ensure_shadows(fwd):
 
 
 def refresh_weight_shadows(fwd):
-    """(Re)build the bf16 copies from the fp32 master (init, rollback, snapshot load)."""
+    """(Re)build the bf16 (and fp8) copies from the fp32 master (init, rollback, snapshot load)."""
     if not fwd.weights or not lp_enabled(fwd):
         return
     ensure_shadows(fwd)
@@ -145,6 +145,89 @@ def refresh_weight_shadows(fwd):
     _ext(fwd).refresh_shadows(fwd.weights.dev, rows, cols, fwd.weights_lp_, ld,
                               fwd.weights_lp_t_ if is_conv else None, taps, c, c_pad,
                               lp_cpad(fwd))
+    _launch()
+    if _fp8_layer(fwd):
+        requantize_weights(fwd)
+
+
+# ------------------------------------------------------------------------------------------
+# fp8 (compute_type "fp8"): fully connected products on block-scaled e4m3 operands
+# (csrc/fp8.cu quantisers + the fp8 mode of csrc/gemm_pair.cu; numerics: utils/mxfp8.py)
+# ------------------------------------------------------------------------------------------
+def _fp8_decline(unit, why):
+    """Record that an fp8-mode product of this unit runs on the bf16 path instead."""
+    _path(unit, "fp8:declined(%s)" % why)
+    key = (id(unit), "fp8:" + why)
+    if key not in _WARNED:
+        _WARNED.add(key)
+        unit.warning("fp8 declined (%s): this product uses the bf16 path", why)
+
+
+def _fp8_layer(fwd):
+    """True when the fully connected unit ``fwd`` runs its products in fp8 (a decline is recorded)."""
+    from ..ops.nn_units import compute_dtype_name
+    if compute_dtype_name() != "fp8" or not fwd.weights:
+        return False
+    from ..ops.all2all import All2All, All2AllSoftmax
+    if not isinstance(fwd, All2All):
+        return False                # convolutions (and LSTM cells) stay bf16 under "fp8"
+    n_out, n_in = fwd.weights.shape
+    if fwd.weights_transposed:
+        why = "weights_transposed"
+    elif n_out <= FC_SMALL_MAX_OUT:
+        why = "fc_small"
+    elif n_in % 16:
+        why = "n_in % 16"
+    elif n_out % (4 if isinstance(fwd, All2AllSoftmax) else 8):
+        why = "output row pitch"    # the TMA-store epilogue writes 16-byte aligned rows (bf16;
+                                    # the softmax layer's logits are fp32)
+    else:
+        return True
+    _fp8_decline(fwd, why)
+    return False
+
+
+def requantize_weights(fwd):
+    """W_q [n_out][n_in16], W_qt [n_in][n_out16] and their expanded tile scales from the fp32
+    master: one launch (init, rollback, broadcast and after every weight update)."""
+    n_out, n_in = fwd.weights.shape
+    dev = fwd.device.torch_device
+    q = fwd.__dict__.get("weights_q_")
+    if q is None or tuple(q.shape) != (n_out, _roundup(n_in, 16)):
+        kb_in, kb_out = -(-n_in // 128), -(-n_out // 128)
+        fwd.weights_q_ = torch.empty((n_out, _roundup(n_in, 16)), dtype=torch.uint8, device=dev)
+        fwd.weights_qt_ = torch.empty((n_in, _roundup(n_out, 16)), dtype=torch.uint8, device=dev)
+        fwd.weights_qs_ = torch.empty((kb_in, kb_out * 128), dtype=torch.float32, device=dev)
+        fwd.weights_qts_ = torch.empty((kb_out, kb_in * 128), dtype=torch.float32, device=dev)
+    r = _ext(fwd).fp8_quant(fwd.weights.dev, n_out, n_in, 1, fwd.weights_q_, fwd.weights_qs_,
+                            fwd.weights_qt_, fwd.weights_qts_)
+    if r != 0:
+        raise RuntimeError("%s: fp8 weight quantiser refused (code %d)" % (fwd, r))
+    _launch()
+
+
+def _fp8_quant_act(unit, ext, name, t, rows, cols, rows_form, cols_form):
+    """bf16 t [rows][cols] -> (q, s) row-block codes and / or (qt, st) transposed codes in
+    buffers cached on the unit (None for a form not asked for)."""
+    kr, kc = -(-rows // 128), -(-cols // 128)
+    q = s = qt = st = None
+    if rows_form:
+        q = _tmp(unit, name + "_q", (rows, _roundup(cols, 16)), torch.uint8)
+        s = _tmp(unit, name + "_s", (kc, kr * 128), torch.float32)
+    if cols_form:
+        qt = _tmp(unit, name + "_qt", (cols, _roundup(rows, 16)), torch.uint8)
+        st = _tmp(unit, name + "_st", (kr, kc * 128), torch.float32)
+    r = ext.fp8_quant(t, rows, cols, 0, q, s, qt, st)
+    if r != 0:
+        raise RuntimeError("%s: fp8 quantiser refused %s (code %d)" % (unit, name, r))
+    _launch()
+    return q, s, qt, st
+
+
+def _fp8_gemm(unit, ext, what, a, sa, b, sb, out, m, n, k, bias, act, alpha):
+    r = ext.fp8_gemm(a, sa, b, sb, out, m, n, k, bias, act, float(alpha))
+    if r != 0:
+        raise RuntimeError("%s: fp8 FC %s refused the shape (code %d)" % (unit, what, r))
     _launch()
 
 
@@ -184,6 +267,14 @@ def fc_forward(unit, softmax=False):
                              unit.max_idx.dev_out if softmax else None, batch, n_in, n_out,
                              act, bool(softmax), ev_args)
         _launch()
+        return
+    if use_lp and unit.weights_q_ is not None and _fp8_layer(unit):
+        xq, xs, _, _ = _fp8_quant_act(unit, ext, "fp8_x", x, batch, n_in, True, False)
+        _fp8_gemm(unit, ext, "forward", xq, xs, unit.weights_q_, unit.weights_qs_, out, batch,
+                  n_out, n_in, bias, act, 1.0)
+        if softmax:
+            ext.softmax_rows(out, unit.output.dev_out, unit.max_idx.dev_out)
+            _launch()
         return
     if use_lp:
         ensure_shadows(unit)
@@ -342,6 +433,8 @@ def _update(unit, is_bias, grad_buf, nparts, part_stride, rows, cols, g_cpad=0):
                          unit.hyper_dev_, colsums, flags, is_bias, rows, cols, lp, ld, lp_conv,
                          taps, c, c_pad, flag_ptrs, epoch_ptr, rank, blocks, cpad_lp, g_cpad)
         _launch()
+        if not is_bias and getattr(fwd, "weights_q_", None) is not None:
+            requantize_weights(fwd)
     w.dev_written()
     if acc:
         acc.dev_written()
@@ -362,6 +455,8 @@ def fc_backward(unit):
     need_b = need_w and unit.include_bias and unit.bias
     if (_fc_small_ok(unit, n_out) and eff_act(unit) <= 4 and err.dtype == x.dtype and
             (eff_act(unit) == ACT_LINEAR or unit.output.dev.dtype == err.dtype)):
+        if unit.forward_unit is not None:
+            _fp8_layer(unit.forward_unit)      # (records the fc_small decline in fp8 mode)
         # whole GD step of a few-output layer in one launch (+ the deferred update)
         bsplit = max(1, min(16, batch // 8))
         gbuf = _grad_buffer(unit, "wgrad", (bsplit,) + tuple(unit.weights.shape)) \
@@ -395,6 +490,17 @@ def fc_backward(unit):
     lp_ok = (lp_enabled(unit) and _is_bf16(err) and _is_bf16(x) and
              unit.forward_unit is not None and
              getattr(unit.forward_unit, "weights_lp_", None) is not None)
+    fwd = unit.forward_unit
+    fp8 = lp_ok and getattr(fwd, "weights_q_", None) is not None and _fp8_layer(fwd)
+    fp8_dgrad = fp8 and unit.need_err_input and not unit.err_input_beta
+    if fp8 and unit.need_err_input and unit.err_input_beta:
+        _fp8_decline(unit, "err_input_beta")
+    eq = es8 = eqt = est = None
+    if fp8_dgrad or (fp8 and need_w):
+        # err (after f' and the bias sums): 1 x 128 blocks along n_out for dgrad, transposed
+        # with blocks along the batch for wgrad - one pass over err for both
+        eq, es8, eqt, est = _fp8_quant_act(unit, ext, "fp8_err", err, batch, n_out, fp8_dgrad,
+                                           fp8 and need_w)
     # the weight-gradient GEMM runs beside the err_input GEMM (see _fork_side)
     x3 = ((not lp_ok) and fp32x.enabled(unit) and fp32x._f32(err, x) and n_in >= 32 and
           n_out >= 32)
@@ -409,6 +515,11 @@ def fc_backward(unit):
         if x3 and fp32x.fc_dgrad(unit, ext, ec, ei, batch, n_in, n_out, unit.err_input_alpha,
                                  unit.err_input_beta):
             pass
+        elif fp8_dgrad:
+            r = ext.fp8_gemm(eq, es8, fwd.weights_qt_, fwd.weights_qts_, ei, batch, n_in, n_out,
+                             None, 0, float(unit.err_input_alpha))
+            if r != 0:
+                raise RuntimeError("%s: fp8 FC dgrad refused the shape (code %d)" % (unit, r))
         elif lp_ok and n_out % 8 == 0:
             w = unit.forward_unit.weights_lp_
             r = ext.gemm(err, n_out, False, w, w.shape[1], False, ei, n_in, False,
@@ -435,7 +546,13 @@ def fc_backward(unit):
     gbuf = _grad_buffer(unit, "wgrad", (1,) + tuple(unit.weights.shape))
     with (torch.cuda.stream(side) if side is not None else contextlib.nullcontext()):
         r = -1
-        if lp_ok and n_out % 8 == 0 and n_in % 8 == 0 and n_out >= 256 and n_in >= 256 \
+        if fp8:
+            _, _, xqt, xst = _fp8_quant_act(unit, ext, "fp8_xt", x, batch, n_in, False, True)
+            r = ext.fp8_gemm(eqt, est, xqt, xst, gbuf.view(n_out, n_in), n_out, n_in, batch,
+                             None, 0, 1.0)
+            if r != 0:
+                raise RuntimeError("%s: fp8 FC wgrad refused the shape (code %d)" % (unit, r))
+        elif lp_ok and n_out % 8 == 0 and n_in % 8 == 0 and n_out >= 256 and n_in >= 256 \
                 and batch >= 64:
             # large layers: err^T . x on the persistent kernel (both operands MN-major,
             # TMA-store epilogue straight into the [neurons][in] gradient layout)

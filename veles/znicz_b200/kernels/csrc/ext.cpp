@@ -30,6 +30,9 @@ void launch_pull_from_host(const void*, void*, long long, cudaStream_t);
 void launch_fp8_absmax(const void*, bool, long long, float*, cudaStream_t);
 void launch_fp8_quantize(const void*, bool, unsigned char*, long long, const float*, cudaStream_t);
 int launch_gemm_fp8(const void*, long long, const void*, long long, void*, int, long long, int, int, int, const float*, int, float, cudaStream_t);
+int launch_fp8_quant(const void*, int, long long, int, int, int, uint8_t*, long long, float*, uint8_t*, long long, float*, cudaStream_t);
+int launch_gemm_fp8_block(const void*, long long, const float*, const void*, long long, const float*, void*, int, long long, int, int, int, const float*, int, float, cudaStream_t);
+long long fp8_gemm_launches();
 void launch_swap01_2d(const void*, int, int, void*, int, int, int, int, int, bool, cudaStream_t);
 void launch_pull_from_host_bytes(const void*, void*, int, cudaStream_t);
 void launch_pool_backward(const void*, const int*, void*, int, int, int, int, int, int, int, int, int, int, int, bool, const void*, int, const void*, int, cudaStream_t);
@@ -350,6 +353,58 @@ int64_t gemm_fp8(Tensor a, Tensor b, Tensor out, c10::optional<Tensor> bias, int
   TORCH_CHECK(out.numel() == (int64_t)M * N);
   int r = zn::launch_gemm_fp8(a.data_ptr(), K, b.data_ptr(), K, out.data_ptr(), is_bf16(out) ? 1 : 0, N, M, N, K,
                               fptr_or_null(bias), (int)act, (float)alpha, cur());
+  if (r == 0) kcheck();
+  return r;
+}
+// ---- block-scaled fp8 (compute_type "fp8"): quantisers of fp8.cu + the fp8 mode of gemm_pair.cu
+static uint8_t* codes_or_null(const c10::optional<Tensor>& t, long long* ld) {
+  if (!t.has_value() || !t->defined()) return nullptr;
+  TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->dim() == 2 && t->element_size() == 1,
+              "fp8 codes: contiguous 2-D 1-byte tensor");
+  *ld = t->size(1);
+  return reinterpret_cast<uint8_t*>(t->data_ptr());
+}
+static float* scales_or_null(const c10::optional<Tensor>& t, long long need) {
+  if (!t.has_value() || !t->defined()) return nullptr;
+  TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == torch::kFloat32 && t->numel() >= need,
+              "fp8 scales: contiguous fp32 tensor of ", need, " elements");
+  return t->data_ptr<float>();
+}
+// x [rows][cols] (bf16, or fp32 with tile = 1) -> row-block codes q [rows][ldq] + scales
+// sq [ceil(cols / 128)][round_up(rows, 128)] and / or transposed codes qt [cols][ldqt] + scales
+// sqt [ceil(rows / 128)][round_up(cols, 128)]; tile = 1: one scale per 128 x 128 tile
+int64_t fp8_quant(Tensor x, int64_t rows, int64_t cols, int64_t tile, c10::optional<Tensor> q,
+                  c10::optional<Tensor> sq, c10::optional<Tensor> qt, c10::optional<Tensor> sqt) {
+  chk(x, "x");
+  TORCH_CHECK(x.numel() == rows * cols, "x: rows x cols elements");
+  const long long rp = (rows + 127) / 128 * 128, cp = (cols + 127) / 128 * 128;
+  long long ldq = 0, ldqt = 0;
+  uint8_t* qp = codes_or_null(q, &ldq);
+  uint8_t* qtp = codes_or_null(qt, &ldqt);
+  if (qp) TORCH_CHECK(q->size(0) == rows, "q: [rows][ldq]");
+  if (qtp) TORCH_CHECK(qt->size(0) == cols, "qt: [cols][ldqt]");
+  float* sqp = qp ? scales_or_null(sq, cp / 128 * rp) : nullptr;
+  float* sqtp = qtp ? scales_or_null(sqt, rp / 128 * cp) : nullptr;
+  int r = zn::launch_fp8_quant(x.data_ptr(), is_bf16(x) ? 0 : 1, cols, (int)rows, (int)cols, (int)tile,
+                               qp, ldq, sqp, qtp, ldqt, sqtp, cur());
+  if (r == 0) kcheck();
+  return r;
+}
+// out[M][N] = act(alpha * sum_kb sa[kb][m] sb[kb][n] (a_kb . b_kb^T) + bias): a [M][lda], b [N][ldb]
+// e4m3 codes, scales as written by fp8_quant. Returns 0, or non-zero when refused.
+int64_t fp8_gemm(Tensor a, Tensor sa, Tensor b, Tensor sb, Tensor out, int64_t M, int64_t N, int64_t K,
+                 c10::optional<Tensor> bias, int64_t act, double alpha) {
+  long long lda = 0, ldb = 0;
+  const uint8_t* ap = codes_or_null(a, &lda);
+  const uint8_t* bp = codes_or_null(b, &ldb);
+  TORCH_CHECK(ap && bp && a.size(0) >= M && b.size(0) >= N, "fp8 operands [M][lda], [N][ldb]");
+  const long long kb = (K + 127) / 128;
+  const float* sap = scales_or_null(sa, kb * ((M + 127) / 128 * 128));
+  const float* sbp = scales_or_null(sb, kb * ((N + 127) / 128 * 128));
+  chk(out, "out");
+  TORCH_CHECK(out.numel() == M * N, "out: M x N elements");
+  int r = zn::launch_gemm_fp8_block(ap, lda, sap, bp, ldb, sbp, out.data_ptr(), is_bf16(out) ? 0 : 1, N,
+                                    (int)M, (int)N, (int)K, fptr_or_null(bias), (int)act, (float)alpha, cur());
   if (r == 0) kcheck();
   return r;
 }
@@ -1044,6 +1099,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("stream_ring_step", &stream_ring_step); m.def("stream_ring_slot_done", &stream_ring_slot_done);
   m.def("stream_ring_slot_sync", &stream_ring_slot_sync);
   m.def("fp8_absmax", &fp8_absmax); m.def("fp8_quantize", &fp8_quantize); m.def("gemm_fp8", &gemm_fp8);
+  m.def("fp8_quant", &fp8_quant); m.def("fp8_gemm", &fp8_gemm);
+  m.def("fp8_gemm_launches", []() { return (int64_t)zn::fp8_gemm_launches(); });
   m.def("pull_from_host", &pull_from_host); m.def("push_to_host", &push_to_host);
   m.def("host_gather_rows", &host_gather_rows);
   m.def("host_prefetch_submit", &host_prefetch_submit);

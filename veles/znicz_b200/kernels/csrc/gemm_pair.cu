@@ -14,6 +14,17 @@
 //
 // Used for the large fully-connected layers and convolutions; skinny / small shapes stay on
 // gemm_umma.cu.
+//
+// fp8 operand mode (AM_FP8, BN = 128 only): A [M][K] and B [N][K] hold e4m3 codes with one fp32
+// scale per row and 128-element k-block (scales [KB][rows rounded up to 128], written by fp8.cu):
+//
+//   D[m, n] = act(alpha * sum_kb sA[kb][m] sB[kb][n] P_kb[m, n] + bias[n])
+//
+// One stage is one k-block (128 e4m3 = one 128-byte SW128 row); the producer also fetches the
+// stage's 2 x 128 scales with two bulk copies. Each MMA warpgroup issues four wgmma m64n128k32
+// e4m3 into a temporary fragment P_kb (the tensor core's partial sums never span more than one
+// k-block), waits, and promotes sA sB P_kb into its fp32 accumulators with one FMA per element.
+// Any M, N, K >= 1: the tails arrive as TMA zero fill.
 #include "common.cuh"
 #include "umma.cuh"
 #include <stdlib.h>
@@ -35,7 +46,8 @@ constexpr int THREADS = 384;
 // im2col mode (one [128 pixels x 64 channels] box per k-block): fprop = im2col(x), dgrad
 // (unit stride) = windows of err_out for the flipped filter.
 enum { AM_DENSE = 0, AM_IM2COL_FPROP = 1, AM_IM2COL_DGRAD = 2,
-       AM_DENSE_MN = 3 };          // A stored [K][M] (M contiguous): err^T of the weight-gradient GEMMs
+       AM_DENSE_MN = 3,            // A stored [K][M] (M contiguous): err^T of the weight-gradient GEMMs
+       AM_FP8 = 4 };               // A, B: block-scaled e4m3 [rows][K] (see the top of the file)
 // B operand: K-major tile, MN-major tile ([K][N], N contiguous), or - conv wgrad - the im2col
 // operand as MN-major blocks fetched by TMA im2col ([64 pixels][64 channels of one tap])
 enum { BM_K = 0, BM_MN = 1, BM_IM2COL_MN = 2 };
@@ -49,6 +61,8 @@ struct Params {
   int splits, kb_per_split;       // split-K over the reduction (fp32 partials [splits][M][N])
   ConvP g;
   const __nv_bfloat16* dmul; int dact; long long ldo;   // dgrad: out *= f'(dmul[row][col])
+  const float* sa; const float* sb;                      // fp8: scales [KB][sa_pitch], [KB][sb_pitch]
+  int sa_pitch, sb_pitch;
 };
 
 __device__ __forceinline__ void tma_store_wait_read(int keep) {
@@ -72,8 +86,14 @@ __device__ __forceinline__ void static_for(std::integer_sequence<int, I...>, F&&
   (f(std::integral_constant<int, I>{}), ...);
 }
 
-template <int BN>
-__host__ __device__ constexpr int pair_stages() { return BN == 256 ? 4 : 6; }
+template <int BN, int AMODE = AM_DENSE>
+__host__ __device__ constexpr int pair_stages() { return AMODE == AM_FP8 ? 5 : (BN == 256 ? 4 : 6); }
+// dynamic shared memory: stages, two epilogue staging buffers, fp8 scales (1 KB per stage), alignment
+template <int BN, int AMODE>
+__host__ __device__ constexpr int pair_smem() {
+  return pair_stages<BN, AMODE>() * (A_BYTES + BN * 128 + (AMODE == AM_FP8 ? 1024 : 0)) + 2 * EPI_BUF +
+         1024;
+}
 
 template <int BN, bool OUT_F32, int AMODE = AM_DENSE, int BMODE = BM_K>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -81,12 +101,15 @@ gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             const __grid_constant__ CUtensorMap tmap_c, const Params p) {
   constexpr int B_BYTES = BN * 128;
   constexpr int STAGE = A_BYTES + B_BYTES;
-  constexpr int NST = pair_stages<BN>();
+  constexpr int NST = pair_stages<BN, AMODE>();
   constexpr int EPI_COLS = OUT_F32 ? 32 : 64;          // 128-byte staging rows
   constexpr int NCHUNK = BN / EPI_COLS;
   constexpr int ESZ = OUT_F32 ? 4 : 2;
   constexpr bool A_MN = (AMODE == AM_DENSE_MN);
   constexpr bool B_MN = (BMODE != BM_K);
+  constexpr bool FP8 = (AMODE == AM_FP8);
+  constexpr int KSTEP = FP8 ? 128 : BK;                 // reduction elements per stage
+  static_assert(!FP8 || (BN == 128 && BMODE == BM_K), "fp8 mode: BN = 128, K-major B");
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[NST];
@@ -95,15 +118,17 @@ gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   uint8_t* tiles = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* epi = tiles + (size_t)NST * STAGE;          // 2 x EPI_BUF, 1024-byte aligned
+  uint8_t* scl = epi + 2 * EPI_BUF;                    // fp8: per stage sA[128] then sB[128]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
   const int splits = p.splits > 1 ? p.splits : 1;
   const int num_tiles = p.tiles_m * p.tiles_n * splits;      // work items (tile, k-split)
-  const int total_kb = (p.K + BK - 1) / BK;
+  const int total_kb = (p.K + KSTEP - 1) / KSTEP;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 2u); }
+    // fp8 mode: every consumer warp releases the stage (it also read the stage's scales)
+    for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], FP8 ? 8u : 2u); }
     fence_barrier_init();
     tma_prefetch_desc(&tmap_a); tma_prefetch_desc(&tmap_b); tma_prefetch_desc(&tmap_c);
   }
@@ -133,8 +158,13 @@ gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             nblk = left <= 0 ? 0 : min(BN / 64, (left + 63) / 64);
             tx = A_BYTES + (uint32_t)nblk * 8192u;
           }
+          if (FP8) tx += 1024;
           mbar_arrive_expect_tx(&full_bar[s], tx);
-          if (AMODE == AM_DENSE) {
+          if (FP8) {
+            tma_load_2d(sa, &tmap_a, &full_bar[s], kb * KSTEP, m0);
+            bulk_load(scl + s * 1024, p.sa + (long long)kb * p.sa_pitch + m0, 512, &full_bar[s]);
+            bulk_load(scl + s * 1024 + 512, p.sb + (long long)kb * p.sb_pitch + n0, 512, &full_bar[s]);
+          } else if (AMODE == AM_DENSE) {
             tma_load_2d(sa, &tmap_a, &full_bar[s], kb * BK, m0);
           } else if (AMODE == AM_DENSE_MN) {
             // A stored [K][M]: two [64 k][64 m] boxes for the tile's 128 rows
@@ -160,7 +190,7 @@ gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             tma_load_im2col_4d(sa, &tmap_a, &full_bar[s], c0, w0, h0, n, (uint16_t)ow, (uint16_t)oh);
           }
           if (BMODE == BM_K) {
-            tma_load_2d(sa + A_BYTES, &tmap_b, &full_bar[s], kb * BK, n0);
+            tma_load_2d(sa + A_BYTES, &tmap_b, &full_bar[s], kb * KSTEP, n0);
           } else if (BMODE == BM_MN) {
             // B stored [K][N] (N contiguous): 64 x 64 boxes, one per 64 columns of the tile
 #pragma unroll
@@ -205,6 +235,36 @@ gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     const int m0 = tm * BM, n0 = tn * BN;
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+    if constexpr (FP8) {
+      float tmp[BN / 2];
+      for (int kb = kb0; kb < kb1; ++kb, ++it) {
+        const int s = it % NST; const uint32_t ph = (it / NST) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE) + half * 8192;
+        const uint32_t sb = smem_u32(tiles + (size_t)s * STAGE) + A_BYTES;
+        const float* ss = reinterpret_cast<const float*>(scl + s * 1024);
+        wg_fence();
+        const uint64_t da = make_smem_desc(sa, 16, 1024), db = make_smem_desc(sb, 16, 1024);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)        // P_kb = sum of four k32 products, from zero
+          wgmma_e4m3_n128(tmp, da + 2 * k, db + 2 * k, k > 0);   // +32 bytes per k32 step
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_regs(tmp);
+        const float a0 = ss[lr], a1 = ss[lr + 8];
+        // (scales of B read inside the loop: holding all 32 across the wait spills)
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+          const float2 b = *reinterpret_cast<const float2*>(ss + 128 + 8 * i + cq);
+          acc[4 * i + 0] = fmaf(a0 * b.x, tmp[4 * i + 0], acc[4 * i + 0]);
+          acc[4 * i + 1] = fmaf(a0 * b.y, tmp[4 * i + 1], acc[4 * i + 1]);
+          acc[4 * i + 2] = fmaf(a1 * b.x, tmp[4 * i + 2], acc[4 * i + 2]);
+          acc[4 * i + 3] = fmaf(a1 * b.y, tmp[4 * i + 3], acc[4 * i + 3]);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
+      }
+    } else {
     for (int kb = kb0; kb < kb1; ++kb, ++it) {
       const int s = it % NST; const uint32_t ph = (it / NST) & 1;
       mbar_wait(&full_bar[s], ph);
@@ -228,6 +288,7 @@ gemm_pair_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     wg_wait<0>();
     wg_fence_regs(acc);
     if (kb1 > kb0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it - 1) % NST]);
+    }
 
     // ---- epilogue: registers -> swizzled staging chunk -> one TMA store per chunk ----
     // split-K partial s lives at rows [s * M, (s + 1) * M) of the output map
@@ -315,7 +376,7 @@ static int make_map(CUtensorMap* m, const void* ptr, CUtensorMapDataType dt, int
 template <int BN, bool OUT_F32, int AMODE = AM_DENSE, int BMODE = BM_K>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const Params& p,
                   cudaStream_t st) {
-  constexpr int smem = pair_stages<BN>() * (A_BYTES + BN * 128) + 2 * EPI_BUF + 1024;
+  constexpr int smem = pair_smem<BN, AMODE>();
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_pair_k<BN, OUT_F32, AMODE, BMODE>,
@@ -364,6 +425,8 @@ static bool conv_pair_enabled() {
   if (on < 0) { const char* e = getenv("ZNICZ_CONV_PAIR"); on = (e && atoi(e) == 0) ? 0 : 1; }
   return on != 0;
 }
+
+static long long g_fp8_launches = 0;
 
 }  // namespace pr
 
@@ -532,5 +595,42 @@ int launch_gemm_pair(const void* a, long long lda, const void* b, long long ldb,
   if (bn == 256) return out_f32 ? launch<256, true>(ta, tb, tc, p, st) : launch<256, false>(ta, tb, tc, p, st);
   return out_f32 ? launch<128, true>(ta, tb, tc, p, st) : launch<128, false>(ta, tb, tc, p, st);
 }
+
+// Block-scaled fp8 GEMM (AM_FP8 mode): out[M][ldo] (bf16 or fp32) = act(alpha * A . B^T + bias),
+// a [M][lda] and b [N][ldb] e4m3 codes (K contiguous), sa [ceil(K / 128)][round_up(M, 128)] and
+// sb [ceil(K / 128)][round_up(N, 128)] their fp32 scales. Any M, N, K >= 1. Returns 0, or non-zero
+// when the shape / alignment is refused (nothing launched).
+int launch_gemm_fp8_block(const void* a, long long lda, const float* sa, const void* b, long long ldb,
+                          const float* sb, void* out, int out_f32, long long ldo, int M, int N, int K,
+                          const float* bias, int act, float alpha, cudaStream_t st) {
+  using namespace pr;
+  const int esz = out_f32 ? 4 : 2;
+  if (M < 1 || N < 1 || K < 1 || lda < K || ldb < K || ldo < N) return -6;
+  if ((lda % 16) || (ldb % 16) || ((uintptr_t)a & 15) || ((uintptr_t)b & 15)) return -3;
+  if (((uintptr_t)sa & 15) || ((uintptr_t)sb & 15) || !sa || !sb) return -3;
+  if (((ldo * esz) % 16) || ((uintptr_t)out & 15)) return -3;
+  constexpr int bn = 128;
+  CUtensorMap ta, tb, tc;
+  int r = make_map(&ta, a, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, K, M, lda, 128, BM);
+  if (r) return r;
+  r = make_map(&tb, b, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, K, N, ldb, 128, bn);
+  if (r) return r;
+  r = make_map(&tc, out, out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, esz,
+               N, M, ldo, out_f32 ? 32 : 64, BM);
+  if (r) return r;
+  Params p{};
+  p.M = M; p.N = N; p.K = K; p.bias = bias; p.act = act; p.alpha = alpha;
+  p.tiles_m = (M + BM - 1) / BM;
+  p.tiles_n = (N + bn - 1) / bn;
+  p.splits = 1; p.kb_per_split = (K + 127) / 128;
+  p.ldo = ldo;
+  p.sa = sa; p.sb = sb;
+  p.sa_pitch = p.tiles_m * BM; p.sb_pitch = p.tiles_n * bn;
+  r = out_f32 ? launch<128, true, AM_FP8, BM_K>(ta, tb, tc, p, st)
+              : launch<128, false, AM_FP8, BM_K>(ta, tb, tc, p, st);
+  if (r == 0) ++g_fp8_launches;
+  return r;
+}
+long long fp8_gemm_launches() { return pr::g_fp8_launches; }
 
 }  // namespace zn

@@ -164,7 +164,7 @@ def build_parser():
                    help="genetic search over Range(...) markers of the config")
     p.add_argument("--dump-config", action="store_true")
     p.add_argument("--no-graphs", action="store_true", help="disable CUDA-graph segments")
-    p.add_argument("--compute", default=None, choices=("fp32", "bf16"))
+    p.add_argument("--compute", default=None, choices=("fp32", "bf16", "fp8"))
     p.add_argument("-v", "--verbosity", default="info",
                    choices=("debug", "info", "warning", "error"))
     return p

@@ -90,7 +90,7 @@ class All2All(nn_units.FullyConnectedOutput, nn_units.NNLayerBase):
         from ..utils import mxfp8
         w = self.weights.mem if self.weights_transposed else self.weights.mem.transpose()
         # (block-scaled fp8 emulation: both operands quantised along the reduction dimension)
-        mem = numpy.dot(mxfp8.operand(self.input.matrix, 1), mxfp8.operand(w, 0))
+        mem = numpy.dot(mxfp8.operand(self.input.matrix, 1), mxfp8.operand(w, 0, tile=True))
         if self.include_bias:
             self.bias.map_read()
             mem += self.bias.mem

@@ -233,6 +233,12 @@ class FusedStep(object):
                                          self.sum_ptrs, getattr(self, "mc_red_used", 0),
                                          self.mc_sum, self.algo, self.max_blocks)
             api._launch()
+        # fp8 layers: their e4m3 weight copies follow the updated fp32 masters (inside the
+        # captured step graph)
+        for e in self.entries:
+            fwd = getattr(e.unit, "forward_unit", None)
+            if e.touched and not e.is_bias and getattr(fwd, "weights_q_", None) is not None:
+                api.requantize_weights(fwd)
         self.launches += 1
         for e in self.entries:
             e.touched = False

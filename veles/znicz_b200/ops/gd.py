@@ -196,7 +196,7 @@ class GradientDescent(GDCommon):
         err_input = self.err_input.matrix
         from ..utils import mxfp8
         w = self.weights.mem.transpose() if self.weights_transposed else self.weights.mem
-        bp = numpy.dot(mxfp8.operand(err_output, 1), mxfp8.operand(w, 0))
+        bp = numpy.dot(mxfp8.operand(err_output, 1), mxfp8.operand(w, 0, tile=True))
         bp *= self.err_input_alpha
         if self.err_input_beta:
             err_input *= self.err_input_beta

@@ -86,6 +86,10 @@ class Forward(ForwardBase):
         super().init_unpickled()
         self.weights_lp_ = None     # bf16 shadow of weights (device)
         self.weights_lp_t_ = None   # transposed bf16 shadow (dgrad operand)
+        self.weights_q_ = None      # fp8 codes W_q / W_qt and their scales (kernels/api.py)
+        self.weights_qt_ = None
+        self.weights_qs_ = None
+        self.weights_qts_ = None
 
     # -- export ------------------------------------------------------------------------
     def package_export(self):

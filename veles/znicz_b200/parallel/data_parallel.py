@@ -60,6 +60,13 @@ class DataParallel(object):
             import datetime
             kw["timeout"] = datetime.timedelta(seconds=float(os.environ.get(
                 "ZNICZ_DP_TIMEOUT_S", root.common.engine.get("dp_timeout_s", 600))))
+            attempt = os.environ.get("TORCHELASTIC_RESTART_COUNT")
+            if attempt is not None and "MASTER_ADDR" in os.environ:
+                # torchrun keeps its store across restarts: without a per-attempt key space a
+                # restarted rank can read the previous attempt's entries (the address of a rank
+                # that has since died) and fail to connect to its peers
+                store, _, _ = next(dist.rendezvous("env://", rank, ws, timeout=kw["timeout"]))
+                kw["store"] = dist.PrefixStore("znicz_attempt_%s" % attempt, store)
             dist.init_process_group(backend=backend, rank=rank, world_size=ws, **kw)
         return cls(device, rank, ws)
 
