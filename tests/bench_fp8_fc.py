@@ -2,8 +2,8 @@
 step through the public API in both compute types. Run on an H100:  python tests/bench_fp8_fc.py
 
 Part 1 times each product with the kernels it needs (CUDA events, L2 flushed before every launch
-group, as tests/bench_fp8_micro.py): forward = [x quantiser +] GEMM, dgrad = [err quantiser (both
-forms) +] GEMM, wgrad = [x^T quantiser +] GEMM, and the per-step fp8 weight re-quantisation.
+group): forward = [x quantiser +] GEMM, dgrad = [err quantiser (both forms) +] GEMM,
+wgrad = [x^T quantiser +] GEMM, and the per-step fp8 weight re-quantisation.
 Part 2 alternates bf16 and fp8 AlexNet training runs (synthetic 227x227 data, batch 128, CUDA
 graphs) and reports ms per step from CUDA events around ``wf.run(iterations=...)``.
 """

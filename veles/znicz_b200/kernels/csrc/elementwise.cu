@@ -4,7 +4,6 @@
 // relu,strict_relu}.cu, dropout.cu, multiplier.cu, summator.cu, cutter.cu,
 // weights_zerofilling.cu. All kernels: grid-stride, 16-byte vector path when aligned.
 #include "common.cuh"
-#include <cuda_fp8.h>
 
 namespace zn {
 
@@ -429,34 +428,6 @@ __global__ void pad_channels_vec_k(const T* __restrict__ x, T* __restrict__ y, l
     }
     st8(y + i * 8, v);
   }
-}
-
-// ---- fp8 (e4m3) per-tensor quantisation: q = sat(x * 448 / amax) -------------------------------
-template <typename T>
-__global__ void absmax_k(const T* __restrict__ x, long long n, float* __restrict__ amax) {
-  pdl_entry();
-  float m = 0.f;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    m = fmaxf(m, fabsf(ldf(x + i)));
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int*>(amax), __float_as_int(m));   // m >= 0
-}
-template <typename T>
-__global__ void quant_e4m3_k(const T* __restrict__ x, unsigned char* __restrict__ q, long long n,
-                             const float* __restrict__ amax) {
-  pdl_entry();
-  const float scale = 448.f / fmaxf(*amax, 1e-12f);
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    q[i] = (unsigned char)__nv_cvt_float_to_fp8(ldf(x + i) * scale, __NV_SATFINITE, __NV_E4M3);
-}
-void launch_fp8_absmax(const void* x, bool bf16, long long n, float* amax, cudaStream_t st) {
-  DISPATCH_T(bf16, launch_k(absmax_k<T>, grid_for(n), 256, 0, st, (const T*)x, n, amax));
-}
-void launch_fp8_quantize(const void* x, bool bf16, unsigned char* q, long long n, const float* amax,
-                         cudaStream_t st) {
-  DISPATCH_T(bf16, launch_k(quant_e4m3_k<T>, grid_for(n), 256, 0, st, (const T*)x, q, n, amax));
 }
 
 void launch_pull_from_host_bytes(const void* src, void* dst, int nbytes, cudaStream_t st) {

@@ -27,9 +27,6 @@ void launch_cast(const void*, bool, void*, bool, long long, cudaStream_t);
 void launch_scatter_offsets(const void*, const int*, void*, long long, bool, cudaStream_t);
 void launch_pool_forward(const void*, void*, int*, int, int, int, int, int, int, int, int, int, int, int, const int*, bool, int, cudaStream_t);
 void launch_pull_from_host(const void*, void*, long long, cudaStream_t);
-void launch_fp8_absmax(const void*, bool, long long, float*, cudaStream_t);
-void launch_fp8_quantize(const void*, bool, unsigned char*, long long, const float*, cudaStream_t);
-int launch_gemm_fp8(const void*, long long, const void*, long long, void*, int, long long, int, int, int, const float*, int, float, cudaStream_t);
 int launch_fp8_quant(const void*, int, long long, int, int, int, uint8_t*, long long, float*, uint8_t*, long long, float*, cudaStream_t);
 int launch_gemm_fp8_block(const void*, long long, const float*, const void*, long long, const float*, void*, int, long long, int, int, int, const float*, int, float, cudaStream_t);
 long long fp8_gemm_launches();
@@ -328,33 +325,6 @@ void device_copy(Tensor src, Tensor dst) {
   TORCH_CHECK((((uintptr_t)src.data_ptr() | (uintptr_t)dst.data_ptr()) & 15) == 0, "16-byte alignment");
   zn::launch_pull_from_host(src.data_ptr(), dst.data_ptr(), nbytes, cur());
   kcheck();
-}
-// ---- fp8: per-tensor e4m3 quantisation + wgmma e4m3 GEMM (first slice of the fp8 path)
-void fp8_absmax(Tensor x, Tensor amax) {
-  chk(x, "x");
-  TORCH_CHECK(amax.is_cuda() && amax.scalar_type() == torch::kFloat32 && amax.numel() >= 1);
-  zn::launch_fp8_absmax(x.data_ptr(), is_bf16(x), x.numel(), amax.data_ptr<float>(), cur());
-  kcheck();
-}
-void fp8_quantize(Tensor x, Tensor q, Tensor amax) {
-  chk(x, "x");
-  TORCH_CHECK(q.is_cuda() && q.is_contiguous() && q.element_size() == 1 && q.numel() == x.numel(), "q: 1-byte tensor of the same size");
-  TORCH_CHECK(amax.is_cuda() && amax.scalar_type() == torch::kFloat32 && amax.numel() >= 1);
-  zn::launch_fp8_quantize(x.data_ptr(), is_bf16(x), reinterpret_cast<unsigned char*>(q.data_ptr()), x.numel(),
-                          amax.data_ptr<float>(), cur());
-  kcheck();
-}
-// out[M][N] = act(alpha * a[M][K] . b[N][K]^T + bias); a, b hold e4m3 bytes (row pitch % 16 == 0)
-int64_t gemm_fp8(Tensor a, Tensor b, Tensor out, c10::optional<Tensor> bias, int64_t act, double alpha) {
-  TORCH_CHECK(a.is_cuda() && b.is_cuda() && a.is_contiguous() && b.is_contiguous() && a.dim() == 2 && b.dim() == 2);
-  TORCH_CHECK(a.element_size() == 1 && b.element_size() == 1 && a.size(1) == b.size(1), "e4m3 operands [M][K], [N][K]");
-  chk(out, "out");
-  const int M = (int)a.size(0), N = (int)b.size(0), K = (int)a.size(1);
-  TORCH_CHECK(out.numel() == (int64_t)M * N);
-  int r = zn::launch_gemm_fp8(a.data_ptr(), K, b.data_ptr(), K, out.data_ptr(), is_bf16(out) ? 1 : 0, N, M, N, K,
-                              fptr_or_null(bias), (int)act, (float)alpha, cur());
-  if (r == 0) kcheck();
-  return r;
 }
 // ---- block-scaled fp8 (compute_type "fp8"): quantisers of fp8.cu + the fp8 mode of gemm_pair.cu
 static uint8_t* codes_or_null(const c10::optional<Tensor>& t, long long* ld) {
@@ -1098,7 +1068,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("stream_ring_create", &stream_ring_create); m.def("stream_ring_destroy", &stream_ring_destroy);
   m.def("stream_ring_step", &stream_ring_step); m.def("stream_ring_slot_done", &stream_ring_slot_done);
   m.def("stream_ring_slot_sync", &stream_ring_slot_sync);
-  m.def("fp8_absmax", &fp8_absmax); m.def("fp8_quantize", &fp8_quantize); m.def("gemm_fp8", &gemm_fp8);
   m.def("fp8_quant", &fp8_quant); m.def("fp8_gemm", &fp8_gemm);
   m.def("fp8_gemm_launches", []() { return (int64_t)zn::fp8_gemm_launches(); });
   m.def("pull_from_host", &pull_from_host); m.def("push_to_host", &push_to_host);

@@ -14,7 +14,7 @@
 // Warp roles: warpgroup 0 (warps 0-3) issues the wgmma for both 64-row halves of the tile, then
 // runs the epilogue (registers -> shared memory -> bias/activation/alpha-beta -> global); its
 // thread 0 issues the TMA loads. Gather kernels add warpgroup 1 (warps 4-7) as producers.
-// 4-stage smem ring.
+// 4-stage smem ring (3 stages for short gather reductions, see launch_cfg).
 //
 // This covers: FC forward (TMA_K x TMA_K, fused bias+activation), FC dgrad (TMA_K x TMA_MN,
 // alpha/beta), FC wgrad (TMA_MN x TMA_MN), conv fprop (GATHER_K x TMA_K, fused bias+act),
@@ -22,24 +22,22 @@
 // that the fused update kernel sums in fixed order).
 #include "common.cuh"
 #include "umma.cuh"
-#include <cuda_fp16.h>
-#include <cuda_fp8.h>
 #include <stdlib.h>
 
 namespace zn {
 
 using namespace umma;
 
-// A_IM2COL_K / A_IM2COL_MN: the same implicit-GEMM operands as A_GATHER_K / A_GATHER_MN, but
-// fetched by TMA in im2col mode (one instruction per [pixels x 64 channels] block instead of a
-// 128-thread LDGSTS gather) - channel counts that are multiples of 64 only.
-enum { A_TMA_K = 0, A_TMA_MN = 1, A_GATHER_K = 2, A_GATHER_MN = 3, A_IM2COL_K = 4, A_IM2COL_MN = 5 };
+// A_IM2COL_K: the same implicit-GEMM operand as A_GATHER_K, but fetched by TMA in im2col mode
+// (one instruction per [128 pixels x 64 channels] block instead of a 128-thread LDGSTS gather) -
+// channel counts that are multiples of 64 only.
+enum { A_TMA_K = 0, A_TMA_MN = 1, A_GATHER_K = 2, A_GATHER_MN = 3, A_IM2COL_K = 4 };
 enum { B_TMA_K = 0, B_TMA_MN = 1 };
 enum { G_NONE = 0, G_IM2COL = 1, G_DGRAD = 2 };
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;          // bf16 elements = 128 bytes = one SW128 row
-constexpr int STAGES_DEFAULT = 4;   // deep (8-stage) variant: see launch_cfg
+constexpr int STAGES_DEFAULT = 4;   // 3 for short gather reductions: see launch_cfg
 constexpr int A_BYTES = BLOCK_M * 128;
 
 struct ConvGeomU {
@@ -68,9 +66,6 @@ struct GemmParams {
   const __nv_bfloat16* gsrc; ConvGeomU g; int gather_kind;
   int gK;                      // valid extent of the gathered K (fprop/dgrad) or M (wgrad) index
   int ktab_n;                  // entries of the gather lookup table (dynamic shared memory)
-  int tma_store;               // epilogue: stage the bf16 tile in smem, one TMA store per warp
-  int dbg;                     // experiments: 1 = producers skip the gather, 2 = skip the MMAs,
-                               // 4 = skip the TMA loads, 8 = skip the epilogue stores, 32 = empty kernel
 };
 
 // ---- gather: 8 consecutive "inner" indices of one "pixel" -> 16 bytes ------------------------
@@ -256,21 +251,6 @@ __host__ __device__ constexpr int b_bytes() {
   return B_MODE == B_TMA_K ? BLOCK_N * 128 : ((BLOCK_N + 63) / 64) * 8192;
 }
 
-// 16 e4m3 bytes -> 16 bf16 (exact: 4 significant bits, exponents within range)
-__device__ __forceinline__ void e4m3x16_to_bf16(uint4 v, uint4& lo, uint4& hi) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-  uint32_t o[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const __nv_fp8x2_storage_t pr = (__nv_fp8x2_storage_t)((w[j >> 1] >> (16 * (j & 1))) & 0xFFFF);
-    const __half2 h = __half2(__nv_cvt_fp8x2_to_halfraw2(pr, __NV_E4M3));
-    const __nv_bfloat162 b = __float22bfloat162_rn(__half22float2(h));
-    o[j] = *reinterpret_cast<const uint32_t*>(&b);
-  }
-  lo = make_uint4(o[0], o[1], o[2], o[3]);
-  hi = make_uint4(o[4], o[5], o[6], o[7]);
-}
-
 // generic (rare) epilogue element: split-K partials, transposed / fp32 / alpha-beta outputs.
 // Deliberately not inlined: keeps the unrolled epilogue small.
 __device__ __noinline__ void epi_store_slow(const GemmParams& p, int row, int n, float v, int z) {
@@ -314,20 +294,16 @@ __host__ __device__ constexpr int min_ctas() {
          : ((2 * (STAGES * (A_BYTES + b_bytes<BLOCK_N, B_MODE>()) + 2048) <= 227 * 1024) ? 2 : 1);
 }
 
-// FP8: operands are e4m3 bytes (TMA / TMA, both K-major): the byte geometry of a stage is the
-// same (128-byte swizzled rows), a k-block is 128 elements and every MMA consumes 32 of them.
-template <int BLOCK_N, int A_MODE, int B_MODE, int GKIND, int GVEC, int STAGES, bool FP8 = false>
+template <int BLOCK_N, int A_MODE, int B_MODE, int GKIND, int GVEC, int STAGES>
 __global__ void __launch_bounds__(kthreads<A_MODE>(), (min_ctas<BLOCK_N, A_MODE, B_MODE, STAGES>()))
 gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-            const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
+            const GemmParams p) {
   pdl_trigger();
   constexpr int B_BYTES = b_bytes<BLOCK_N, B_MODE>();
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr bool A_GATHER = (A_MODE == A_GATHER_K || A_MODE == A_GATHER_MN);
-  constexpr bool A_MN = (A_MODE == A_TMA_MN || A_MODE == A_GATHER_MN || A_MODE == A_IM2COL_MN);
+  constexpr bool A_MN = (A_MODE == A_TMA_MN || A_MODE == A_GATHER_MN);
   constexpr bool B_MN = (B_MODE == B_TMA_MN);
-  constexpr int KBLK = FP8 ? 2 * BLOCK_K : BLOCK_K;      // elements per k-block (128 bytes per row)
-  static_assert(!FP8 || (A_MODE == A_TMA_K && B_MODE == B_TMA_K), "fp8: TMA K-major operands only");
   static_assert(!B_MN || BLOCK_N >= 64, "MN-major B tiles are built from 64-wide swizzle atoms");
   static_assert(stage_f32_bytes<BLOCK_N>() <= STAGES * STAGE_BYTES, "epilogue staging exceeds the ring");
   constexpr uint32_t TX_BYTES = (A_GATHER ? 0 : A_BYTES) + B_BYTES;
@@ -346,15 +322,10 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   // tile's bias slice (the epilogue would otherwise wait on one L2 round trip per 8 columns)
   int* const ktab = reinterpret_cast<int*>(tiles + (size_t)STAGES * STAGE_BYTES);
   float* const s_bias = reinterpret_cast<float*>(ktab + ((p.ktab_n + 3) & ~3));
-  // fp8 only: the stage expanded to bf16, A [2][128 rows][128 B] then B [2][BLOCK_N rows][128 B]
-  uint8_t* const cvt_a = reinterpret_cast<uint8_t*>(
-      (reinterpret_cast<uintptr_t>(s_bias + BLOCK_N) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* const cvt_b = cvt_a + 2 * BLOCK_M * 128;
 
-  if (p.dbg & 32) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.y * BLOCK_M, n0 = blockIdx.x * BLOCK_N;
-  const int total_kb = (p.K + KBLK - 1) / KBLK;
+  const int total_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
   const int kb_begin = blockIdx.z * p.k_blocks_per_split;
   const int kb_end = min(total_kb, kb_begin + p.k_blocks_per_split);
   const int num_kb = max(0, kb_end - kb_begin);
@@ -392,8 +363,7 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           const int s = i % STAGES; const uint32_t ph = (i / STAGES) & 1;
           mbar_wait(&empty_bar[s], ph ^ 1);
           const uint32_t row_base = smem_u32(tiles + (size_t)s * STAGE_BYTES) + t * 128;
-          if (!(p.dbg & 1))
-            gather_row_async<GKIND>(row_base, t & 7, ktab, p.g, ctx, (kb_begin + i) * BLOCK_K);
+          gather_row_async<GKIND>(row_base, t & 7, ktab, p.g, ctx, (kb_begin + i) * BLOCK_K);
           cp_async_mbar_arrive_noinc(&full_bar[s]);
         }
       } else {
@@ -473,27 +443,8 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     const int s = i % STAGES;
     uint8_t* sa = tiles + (size_t)s * STAGE_BYTES;
     uint8_t* sb = sa + A_BYTES;
-    const int k0 = (kb_begin + i) * KBLK;
-    if (p.dbg & 4) { mbar_arrive(&full_bar[s]); return; }
-    if (A_MODE == A_IM2COL_MN) {
-      // conv wgrad: tile = [64 pixels (reduction rows)][128 reduction-weight indices] = two
-      // [64 pixels x 64 channels] im2col boxes (one tap each); a block past Kw is skipped
-      const ConvGeomU& g = p.g;
-      const int pix0 = (kb_begin + i) * BLOCK_K;
-      const int q = pix0 % g.OW; const int t2 = pix0 / g.OW;
-      const int pr = t2 % g.OH; const int n = t2 / g.OH;
-      const int w0 = q * g.SX - g.PL, h0 = pr * g.SY - g.PT;
-      const int nblk = (m0 + 64 < p.gK) ? 2 : 1;
-      mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(B_BYTES + nblk * 8192));
-      for (int mb = 0; mb < nblk; ++mb) {
-        const int kidx0 = m0 + mb * 64;
-        const int tap = kidx0 / g.C, c0 = kidx0 - tap * g.C;
-        tma_load_im2col_4d(sa + mb * 8192, &tmap_a, &full_bar[s], c0, w0, h0, n,
-                           (uint16_t)(tap % g.KX), (uint16_t)(tap / g.KX));
-      }
-    } else {
-      mbar_arrive_expect_tx(&full_bar[s], TX_BYTES);
-    }
+    const int k0 = (kb_begin + i) * BLOCK_K;
+    mbar_arrive_expect_tx(&full_bar[s], TX_BYTES);
     if (A_MODE == A_IM2COL_K) {
       // conv fprop / stride-1 dgrad: tile rows = pixels m0 .. m0 + 127, k-block = 64
       // channels of ONE filter tap
@@ -539,65 +490,20 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     if (A_GATHER && GVEC == 2) fence_proxy_async_smem();   // LDGSTS data -> async proxy
     const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE_BYTES);
     const uint32_t sb = sa + A_BYTES;
-    if constexpr (FP8) {
-      // e4m3 wgmma accumulates with fewer mantissa bits than fp32. Every e4m3 value is exact in
-      // bf16, so the stage is expanded to bf16 tiles in shared memory (two 64-element SW128
-      // k-blocks per 128-byte row) and multiplied with bf16 wgmma: fp8 storage and traffic,
-      // fp32 accumulation.
-      const uint8_t* sa8 = tiles + (size_t)s * STAGE_BYTES;
-      const uint8_t* sb8 = sa8 + A_BYTES;
-      for (int q = threadIdx.x; q < (BLOCK_M + BLOCK_N) * 8; q += 128) {
-        const int rr = q >> 3, c = q & 7;
-        const bool is_a = rr < BLOCK_M;
-        const int r = is_a ? rr : rr - BLOCK_M;
-        const uint4 v = *reinterpret_cast<const uint4*>((is_a ? sa8 : sb8) + r * 128 + ((c ^ (r & 7)) << 4));
-        uint4 lo, hi;
-        e4m3x16_to_bf16(v, lo, hi);
-        uint8_t* d = (is_a ? cvt_a : cvt_b) + (c >> 2) * (is_a ? BLOCK_M : BLOCK_N) * 128 + r * 128;
-        const int c2 = (2 * c) & 7;
-        *reinterpret_cast<uint4*>(d + ((c2 ^ (r & 7)) << 4)) = lo;
-        *reinterpret_cast<uint4*>(d + (((c2 + 1) ^ (r & 7)) << 4)) = hi;
-      }
-      fence_proxy_async_smem();
-      named_bar_sync(1, 128);
-      if (threadIdx.x == 0) {                  // the e4m3 stage is consumed
-        mbar_arrive(&empty_bar[s]);
-        if (i + STAGES < num_kb) issue_loads(i + STAGES);
-      }
-      wg_fence_regs(acc0); wg_fence_regs(acc1);
-      wg_fence();
-      if (!(p.dbg & 2)) {
-#pragma unroll
-        for (int kb2 = 0; kb2 < 2; ++kb2)
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k) {
-            const uint32_t a0 = smem_u32(cvt_a) + kb2 * BLOCK_M * 128 + k * 32;
-            const uint64_t db = make_smem_desc(smem_u32(cvt_b) + kb2 * BLOCK_N * 128 + k * 32, 16, 1024);
-            wgmma_bf16<BLOCK_N, 0, 0>(acc0, make_smem_desc(a0, 16, 1024), db, 1);
-            wgmma_bf16<BLOCK_N, 0, 0>(acc1, make_smem_desc(a0 + 8192, 16, 1024), db, 1);
-          }
-      }
-      wg_commit();
-      wg_wait<0>();                              // (the next stage overwrites the bf16 tiles)
-      wg_fence_regs(acc0); wg_fence_regs(acc1);
-      continue;
-    }
     wg_fence_regs(acc0); wg_fence_regs(acc1);
     wg_fence();
-    if (!(p.dbg & 2)) {
 #pragma unroll
-      for (int k = 0; k < BLOCK_K / 16; ++k) {
-        // K-major: 16 bf16 = 32 B along the swizzled row. MN-major: 16 k-rows = 2 atoms.
-        // The 64-row halves of A are 8192 bytes apart in both layouts.
-        const uint64_t da0 = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024)
-                                  : make_smem_desc(sa + k * 32, 16, 1024);
-        const uint64_t da1 = A_MN ? make_smem_desc(sa + 8192 + k * 2048, 8192, 1024)
-                                  : make_smem_desc(sa + 8192 + k * 32, 16, 1024);
-        const uint64_t db = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024)
-                                 : make_smem_desc(sb + k * 32, 16, 1024);
-        wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc0, da0, db, 1);
-        wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc1, da1, db, 1);
-      }
+    for (int k = 0; k < BLOCK_K / 16; ++k) {
+      // K-major: 16 bf16 = 32 B along the swizzled row. MN-major: 16 k-rows = 2 atoms.
+      // The 64-row halves of A are 8192 bytes apart in both layouts.
+      const uint64_t da0 = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024)
+                                : make_smem_desc(sa + k * 32, 16, 1024);
+      const uint64_t da1 = A_MN ? make_smem_desc(sa + 8192 + k * 2048, 8192, 1024)
+                                : make_smem_desc(sa + 8192 + k * 32, 16, 1024);
+      const uint64_t db = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024)
+                               : make_smem_desc(sb + k * 32, 16, 1024);
+      wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc0, da0, db, 1);
+      wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc1, da1, db, 1);
     }
     wg_commit();
     wg_fence_regs(acc0); wg_fence_regs(acc1);
@@ -631,18 +537,14 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
   }
   named_bar_sync(1, 128);
-  enum { EPI_TMA = 0, EPI_BF16 = 1, EPI_RAW_T = 2, EPI_RAW = 3, EPI_SLOW = 4, EPI_NONE = 5,
-         EPI_BIASROW = 6, EPI_F32 = 7 };
-  uint8_t* const tma_stage = tiles + stage_f32_bytes<BLOCK_N>();
+  enum { EPI_BF16, EPI_RAW_T, EPI_RAW, EPI_SLOW, EPI_NONE, EPI_BIASROW, EPI_F32 };
   {
     const int row = m0 + (int)threadIdx.x;
     const bool raw32 = !p.out_bf16 && p.beta == 0.f && p.alpha == 1.f && !p.bias && p.act == 0;
     float* const rbase = reinterpret_cast<float*>(p.out) +
                          (p.split_stride > 0 ? (long long)blockIdx.z * p.split_stride : 0LL);
     int mode;
-    if (p.tma_store) mode = EPI_TMA;
-    else if (row >= p.M || (p.dbg & 8))
-      mode = (p.bias_out && row == p.M && !(p.dbg & 8)) ? EPI_BIASROW : EPI_NONE;
+    if (row >= p.M) mode = (p.bias_out && row == p.M) ? EPI_BIASROW : EPI_NONE;
     else if (p.split_stride == 0 && !p.out_trans && p.out_bf16 && p.beta == 0.f) mode = EPI_BF16;
     else if (p.split_stride == 0 && !p.out_trans && !p.out_bf16 && p.beta == 0.f && !raw32)
       mode = EPI_F32;        // fp32 row-major with bias / activation (LSTM gate pre-activations,
@@ -662,7 +564,7 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           if (nb + j < p.N) p.bias_out[(long long)blockIdx.z * p.N + nb + j] = __uint_as_float(r[j]);
         return;
       }
-      if (mode == EPI_TMA || mode == EPI_BF16 || mode == EPI_F32) {
+      if (mode == EPI_BF16 || mode == EPI_F32) {
         float v[8];
         {
           const float4 b0 = *reinterpret_cast<const float4*>(s_bias + c0);
@@ -672,8 +574,8 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         }
         // activation selected once per chunk (not per element): the executed path stays short
         switch (p.act) {
-          // out = act(alpha * acc + bias): alpha is the operand de-scaling of the fp8 path and the
-          // err_input_alpha of dgrad (no bias, linear); every other caller passes alpha = 1
+          // out = act(alpha * acc + bias): alpha is the err_input_alpha of dgrad (no bias,
+          // linear); every other caller passes alpha = 1
           case ACT_LINEAR:
 #pragma unroll
             for (int j = 0; j < 8; ++j) v[j] = fmaf(__uint_as_float(r[j]), p.alpha, v[j]);
@@ -692,8 +594,6 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             for (int j = 0; j < 8; ++j)
               v[j] = act_fwd5_fast(p.act, fmaf(__uint_as_float(r[j]), p.alpha, v[j]));
         }
-        // bf16 pack: one 16-byte store per 8 outputs. TMA mode stages the 32 x BLOCK_N sub-tile
-        // of this warp in the (idle by now) pipeline buffers; it leaves with one TMA store below
         if (p.dmul != nullptr && mode == EPI_BF16) {
           // err_input *= f'(x): x has the layout of the output (row pitch ldo)
           const __nv_bfloat16* dx = p.dmul + (long long)row * p.ldo + nb;
@@ -720,11 +620,9 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           }
           return;
         }
-        __nv_bfloat16* q = (mode == EPI_TMA)
-            ? reinterpret_cast<__nv_bfloat16*>(tma_stage + warp * 8192 + lane * (BLOCK_N * 2)) + c0
-            : reinterpret_cast<__nv_bfloat16*>(p.out) + (long long)row * p.ldo + nb;
-        if (mode == EPI_TMA || (nb + 8 <= p.N && (p.ldo & 7) == 0)) {
-          st8(q, v);
+        __nv_bfloat16* q = reinterpret_cast<__nv_bfloat16*>(p.out) + (long long)row * p.ldo + nb;
+        if (nb + 8 <= p.N && (p.ldo & 7) == 0) {
+          st8(q, v);                   // bf16 pack: one 16-byte store per 8 outputs
         } else {                       // ragged last chunk / row pitch not a multiple of 16 bytes
 #pragma unroll
           for (int j = 0; j < 8; ++j)
@@ -755,7 +653,7 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 
 #pragma unroll 1
     for (int c0 = 0; c0 < BLOCK_N; c0 += 8) {
-      if (n0 + c0 >= p.N && mode != EPI_TMA) break;     // chunk beyond the last column
+      if (n0 + c0 >= p.N) break;     // chunk beyond the last column
       uint32_t ra[8];
       const float4 x0 = *reinterpret_cast<const float4*>(srow + c0);
       const float4 x1 = *reinterpret_cast<const float4*>(srow + c0 + 4);
@@ -764,16 +662,6 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       ra[4] = __float_as_uint(x1.x); ra[5] = __float_as_uint(x1.y);
       ra[6] = __float_as_uint(x1.z); ra[7] = __float_as_uint(x1.w);
       emit(ra, c0);
-    }
-    if (p.tma_store) {
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0 && !(p.dbg & 8)) {
-        // rows / columns beyond M / N are clipped by the tensor map
-        tma_store_2d(&tmap_c, tma_stage + warp * 8192, n0, m0 + warp * 32);
-        tma_store_commit_and_wait_read();
-      }
-      __syncwarp();
     }
   }
 }
@@ -856,20 +744,6 @@ static bool im2col_tma_enabled() {
   return on != 0;
 }
 
-// bf16 output tile map for the TMA-store epilogue: dims {N, M}, box {BN, 32}, no swizzle
-static int make_map_out(CUtensorMap* m, const void* ptr, long long N, long long M, long long ldo, int bn) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return -1;
-  cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)M};
-  cuuint64_t strides[1] = {(cuuint64_t)(ldo * 2)};
-  cuuint32_t box[2] = {(cuuint32_t)bn, 32u};
-  cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box,
-                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)r;
-}
-
 template <int BN, int AM, int BM, int GK, int GV, int NS>
 static int launch_stages(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p_in, dim3 grid,
                          cudaStream_t st) {
@@ -890,44 +764,15 @@ static int launch_stages(const CUtensorMap& ta, const CUtensorMap& tb, const Gem
     p.ktab_n = p.g.tpk > 0 ? p.g.ntaps : std::min(KTAB, (p.gK + step - 1) / step);
   }
   const int smem = ring + ((p.ktab_n + 3) & ~3) * 4 + BN * 4;
-  CUtensorMap tc = ta;
-  // TMA-store epilogue (smem staging + one tile store per warp) for plain bf16 row-major outputs,
-  // opt-in with ZNICZ_UMMA_TMA_STORE=1 (the default is the direct 16-byte stores).
-  static int no_tma_store = -1;
-  if (no_tma_store < 0) { const char* e = getenv("ZNICZ_UMMA_TMA_STORE"); no_tma_store = (e && atoi(e)) ? 0 : 1; }
-  p.tma_store = 0;
-  if (!no_tma_store && p.out_bf16 && p.split_stride == 0 && !p.out_trans && p.beta == 0.f &&
-      (p.ldo % 8) == 0 && ((uintptr_t)p.out & 15) == 0 &&
-      stage_f32_bytes<BN>() + 4 * 8192 <= ring - 1024) {
-    if (make_map_out(&tc, p.out, p.N, p.M, p.ldo, BN) == 0) p.tma_store = 1;
-  }
-  launch_k(gemm_umma_k<BN, AM, BM, GK, GV, NS>, grid, kthreads<AM>(), smem, st, ta, tb, tc, p);
+  launch_k(gemm_umma_k<BN, AM, BM, GK, GV, NS>, grid, kthreads<AM>(), smem, st, ta, tb, p);
   return (int)cudaGetLastError();
 }
 
 template <int BN, int AM, int BM, int GK, int GV>
-static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p_in, int splits,
+static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int splits,
                       cudaStream_t st) {
-  GemmParams p = p_in;
-  {
-    static int dbg = -1;
-    if (dbg < 0) { const char* e = getenv("ZNICZ_UMMA_DBG"); dbg = e ? atoi(e) : 0; }
-    p.dbg = dbg;
-  }
   const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
   dim3 grid((p.N + BN - 1) / BN, m_tiles, splits);
-  // Grids that leave one CTA (or none) per SM cannot hide the gather latency by co-residency:
-  // give those CTAs an 8-deep ring instead (asynchronous LDGSTS producers only, and only when
-  // the K loop is long enough to use it).
-  constexpr bool deep_ok = (GV == 2) && (8 * (A_BYTES + b_bytes<BN, BM>()) + 2048 <= 227 * 1024);
-  if constexpr (deep_ok) {
-    const long long ctas = (long long)grid.x * grid.y * grid.z;
-    const int kb = p.k_blocks_per_split;
-    // opt-in with ZNICZ_UMMA_DEEP=1
-    static int deep = -1;
-    if (deep < 0) { const char* e = getenv("ZNICZ_UMMA_DEEP"); deep = e ? atoi(e) : 0; }
-    if (deep && ctas <= num_sms() && kb >= 8) return launch_stages<BN, AM, BM, GK, GV, 8>(ta, tb, p, grid, st);
-  }
   // Short reductions (K <= 4 k-blocks, e.g. a 5x5 first layer on 8 padded channels) in grids of
   // several waves: a 3-stage ring already holds almost the whole K and is small enough for a
   // third CTA per SM (these kernels are latency bound).
@@ -1012,61 +857,6 @@ int launch_gemm_umma(const void* a, long long lda, int a_mn, const void* b, long
   if (!a_mn && b_mn) return launch_bn<A_TMA_K, B_TMA_MN, 0, 0>(bn, ta, tb, p, splits, st);
   if (a_mn && !b_mn) return launch_bn<A_TMA_MN, B_TMA_K, 0, 0>(bn, ta, tb, p, splits, st);
   return launch_bn<A_TMA_MN, B_TMA_MN, 0, 0>(bn, ta, tb, p, splits, st);
-}
-
-// ---- fp8 (e4m3 x e4m3 -> fp32 accumulate) GEMM: out = act(alpha * a . b^T + bias) -------------
-static int make_map_u8(CUtensorMap* m, const void* ptr, long long inner, long long outer, long long ld,
-                       int box_rows) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return -1;
-  cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
-  cuuint64_t strides[1] = {(cuuint64_t)ld};
-  cuuint32_t box[2] = {128u, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box,
-                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : (int)r;
-}
-template <int BN>
-static int launch_fp8_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, dim3 grid,
-                         cudaStream_t st) {
-  constexpr int ring = STAGES_DEFAULT * (A_BYTES + b_bytes<BN, B_TMA_K>()) + 1024;
-  constexpr int smem = ring + BN * 4 + 1024 + 2 * (BLOCK_M + BN) * 128;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_umma_k<BN, A_TMA_K, B_TMA_K, 0, 0, STAGES_DEFAULT, true>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
-  }
-  launch_k(gemm_umma_k<BN, A_TMA_K, B_TMA_K, 0, 0, STAGES_DEFAULT, true>, grid, 128, smem, st, ta, tb, ta, p);
-  return (int)cudaGetLastError();
-}
-// a [M][lda] e4m3, b [N][ldb] e4m3 (both K-major, ld % 16 == 0); alpha carries 1/(scale_a*scale_b)
-int launch_gemm_fp8(const void* a, long long lda, const void* b, long long ldb, void* out, int out_bf16,
-                    long long ldo, int M, int N, int K, const float* bias, int act, float alpha,
-                    cudaStream_t st) {
-  if ((lda % 16) || (ldb % 16) || ((uintptr_t)a & 15) || ((uintptr_t)b & 15)) return -3;
-  CUtensorMap ta, tb;
-  const int bn = pick_bn(N);
-  int r = make_map_u8(&ta, a, K, M, lda, BLOCK_M);
-  if (r) return r;
-  r = make_map_u8(&tb, b, K, N, ldb, bn);
-  if (r) return r;
-  GemmParams p{};
-  p.M = M; p.N = N; p.K = K;
-  p.k_blocks_per_split = (K + 2 * BLOCK_K - 1) / (2 * BLOCK_K);
-  p.out = out; p.out_bf16 = out_bf16; p.ldo = ldo; p.out_trans = 0;
-  p.bias = bias; p.act = act; p.alpha = alpha; p.beta = 0.f; p.split_stride = 0;
-  p.gather_kind = G_NONE;
-  dim3 grid((N + bn - 1) / bn, (M + BLOCK_M - 1) / BLOCK_M, 1);
-  switch (bn) {
-    case 16: return launch_fp8_bn<16>(ta, tb, p, grid, st);
-    case 32: return launch_fp8_bn<32>(ta, tb, p, grid, st);
-    case 64: return launch_fp8_bn<64>(ta, tb, p, grid, st);
-    default: return launch_fp8_bn<128>(ta, tb, p, grid, st);
-  }
 }
 
 static ConvGeomU geom(int N, int H, int W, int C, int OH, int OW, int F, int KY, int KX, int SY, int SX,
@@ -1215,21 +1005,6 @@ int launch_conv_wgrad_umma(const void* err_out, const void* x, float* partials, 
   p.bias = nullptr; p.act = 0; p.alpha = 1.f; p.beta = 0.f; p.split_stride = (long long)F * Kw;
   p.gsrc = (const __nv_bfloat16*)x; p.g = geom(N, H, W, C, OH, OW, F, KY, KX, SY, SX, PT, PL, C % 8 == 0);
   p.gather_kind = G_IM2COL; p.gK = Kw;
-  static int wg_tma = -1;
-  if (wg_tma < 0) { const char* e = getenv("ZNICZ_IM2COL_TMA_WGRAD"); wg_tma = (e && atoi(e)) ? 1 : 0; }
-  // (the LDGSTS gather also delivers the bias row, so the single-CTA TMA form is opt-in; large
-  // layers take the persistent kernel above)
-  if (wg_tma && C % 64 == 0 && im2col_tma_enabled()) {
-    // im2col operand by TMA, 64 pixels x 64 channels per box (no "ones" row here: the caller
-    // computes the bias gradient with the column-sum kernel when this returns 0)
-    CUtensorMap ti;
-    if (make_map_im2col(&ti, x, N, H, W, C, -PL, -PT, (OW - 1) * SX + 1 - PL - W,
-                        (OH - 1) * SY + 1 - PT - H, SX, SY, 64) == 0) {
-      p.g.inner = C;
-      ++g_im2col_launches;
-      return launch_bn<A_IM2COL_MN, B_TMA_MN, G_IM2COL, 0>(bn, ti, tb, p, splits, st);
-    }
-  }
   if (set_tap_mode(p.g, C, false)) {
     bool row = bias_parts != nullptr && (Kw % BLOCK_M) != 0;
     if (row) {
