@@ -51,6 +51,7 @@ int launch_gemm_pair(const void*, long long, const void*, long long, void*, int,
                      const float*, int, float, cudaStream_t);
 long long im2col_tma_launches();
 long long conv_pair_launches();
+long long conv_halo_launches();
 int launch_fc_wgrad_pair(const void*, long long, const void*, long long, float*, long long, int, int, int,
                          cudaStream_t);
 size_t multi_update_desc_size();
@@ -1096,6 +1097,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("fc_wgrad_pair", &fc_wgrad_pair);
   m.def("conv_pair_launches", []() { return (int64_t)zn::conv_pair_launches(); });
   m.def("im2col_tma_launches", []() { return (int64_t)zn::im2col_tma_launches(); });
+  m.def("conv_halo_launches", []() { return (int64_t)zn::conv_halo_launches(); });
   m.def("gemm", &gemm); m.def("pick_splits", &pick_splits); m.def("gemm_pair", &gemm_pair);
   m.def("conv_fprop", &conv_fprop); m.def("conv_dgrad", &conv_dgrad); m.def("conv_wgrad", &conv_wgrad);
 }

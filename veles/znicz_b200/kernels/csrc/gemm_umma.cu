@@ -31,7 +31,15 @@ using namespace umma;
 // A_IM2COL_K: the same implicit-GEMM operand as A_GATHER_K, but fetched by TMA in im2col mode
 // (one instruction per [128 pixels x 64 channels] block instead of a 128-thread LDGSTS gather) -
 // channel counts that are multiples of 64 only.
-enum { A_TMA_K = 0, A_TMA_MN = 1, A_GATHER_K = 2, A_GATHER_MN = 3, A_IM2COL_K = 4 };
+// A_HALO: stride-1 conv fprop / dgrad whose inner channel count is 8, 16 or 32 (tap mode with
+// tpk >= 2). Each 64-row half of the tile is one 8x8 block of output (dgrad: input) pixels; the
+// block's (8 + KY - 1) x (8 + KX - 1) input window is loaded ONCE by TMA into shared memory as
+// planes [C / 8][halo_y][halo_x][8 channels], and every k16 step points a no-swizzle A
+// descriptor into it: a core matrix (8 pixels of one block row x 8 channels) is 128 contiguous
+// bytes of a plane, SBO = one halo row. The tap-mode gather instead fetches each input byte once
+// per filter tap (25x for 5x5). The k16 steps issue the same products in the same order as the
+// gather, so the results are bit-identical.
+enum { A_TMA_K = 0, A_TMA_MN = 1, A_GATHER_K = 2, A_GATHER_MN = 3, A_IM2COL_K = 4, A_HALO = 5 };
 enum { B_TMA_K = 0, B_TMA_MN = 1 };
 enum { G_NONE = 0, G_IM2COL = 1, G_DGRAD = 2 };
 
@@ -39,6 +47,7 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;          // bf16 elements = 128 bytes = one SW128 row
 constexpr int STAGES_DEFAULT = 4;   // 3 for short gather reductions: see launch_cfg
 constexpr int A_BYTES = BLOCK_M * 128;
+constexpr int HALO_MAX_BYTES = 32 * 1024;   // one block's halo (A_HALO), at most
 
 struct ConvGeomU {
   int N, H, W, C, OH, OW, F, KY, KX, SY, SX, PT, PL;
@@ -66,6 +75,8 @@ struct GemmParams {
   const __nv_bfloat16* gsrc; ConvGeomU g; int gather_kind;
   int gK;                      // valid extent of the gathered K (fprop/dgrad) or M (wgrad) index
   int ktab_n;                  // entries of the gather lookup table (dynamic shared memory)
+  // A_HALO: 8x8 pixel blocks per image row / column, and the bytes one block's halo occupies
+  int hnbx, hnby, hbytes;
 };
 
 // ---- gather: 8 consecutive "inner" indices of one "pixel" -> 16 bytes ------------------------
@@ -246,6 +257,46 @@ __device__ __forceinline__ void gather_row(uint4 (&nv)[8], const int* ktab, cons
   }
 }
 
+// ---- A_HALO geometry ---------------------------------------------------------------------------
+// One plane (8 channels) of a block's halo, padded to the 128-byte alignment of a TMA destination.
+__host__ __device__ __forceinline__ int halo_plane_bytes(const ConvGeomU& g) {
+  return ((8 + g.KY - 1) * (8 + g.KX - 1) * 16 + 127) & ~127;
+}
+// Per k16 step s of the reduction: (LBO << 16) | byte offset of the step's first core matrix in a
+// block's halo. The step covers reduction indices 16 s .. 16 s + 15, laid out as the tap-mode
+// gather lays them out: tpk = 8: taps 2 s and 2 s + 1, 8 channels each (LBO = distance between the
+// two taps' windows); tpk = 4: tap s, planes 0 and 1; tpk = 2: tap s / 2, planes 2 (s % 2) and
+// 2 (s % 2) + 1 (LBO = one plane). Padding taps (>= KY * KX, zero rows of B) read the last real
+// tap: finite data, so 0 x A stays 0.
+template <int KIND>
+__device__ __forceinline__ void build_halo_tab(int* tab, const GemmParams& p) {
+  const ConvGeomU& g = p.g;
+  const int hx = 8 + g.KX - 1, plane = halo_plane_bytes(g);
+  auto off = [&](int t) {
+    t = min(t, g.ntaps - 1);
+    int ky = t / g.KX, kx = t - ky * g.KX;
+    if (KIND == G_DGRAD) { ky = g.KY - 1 - ky; kx = g.KX - 1 - kx; }   // correlation, flipped taps
+    return (ky * hx + kx) * 16;
+  };
+  for (int s = threadIdx.x; s < p.ktab_n; s += blockDim.x) {
+    int a, lbo;
+    if (g.tpk == 8) { a = off(2 * s); lbo = off(2 * s + 1) - a; }
+    else if (g.tpk == 4) { a = off(s); lbo = plane; }
+    else { a = (s & 1) * 2 * plane + off(s >> 1); lbo = plane; }
+    tab[s] = (lbo << 16) | a;
+  }
+}
+// GEMM row (output pixel; dgrad: input pixel) of tile row t, or -1 outside the image
+template <int KIND>
+__device__ __forceinline__ int halo_row(const GemmParams& p, int t) {
+  const ConvGeomU& g = p.g;
+  const int b = blockIdx.y * 2 + (t >> 6), r = t & 63;
+  const int bx = b % p.hnbx, b2 = b / p.hnbx, by = b2 % p.hnby, n = b2 / p.hnby;
+  const int PH = KIND == G_IM2COL ? g.OH : g.H, PW = KIND == G_IM2COL ? g.OW : g.W;
+  const int y = by * 8 + (r >> 3), x = bx * 8 + (r & 7);
+  return (n < g.N && y < PH && x < PW) ? (n * PH + y) * PW + x : -1;
+}
+
 template <int BLOCK_N, int B_MODE>
 __host__ __device__ constexpr int b_bytes() {
   return B_MODE == B_TMA_K ? BLOCK_N * 128 : ((BLOCK_N + 63) / 64) * 8192;
@@ -286,11 +337,18 @@ __host__ __device__ constexpr int stage_f32_bytes() {
   return ((BLOCK_M * (BLOCK_N + 4) * 4) + 1023) & ~1023;
 }
 
+// bytes of one ring stage that hold A (the halo kernel keeps A outside the ring)
+template <int A_MODE>
+__host__ __device__ constexpr int a_stage_bytes() { return A_MODE == A_HALO ? 0 : A_BYTES; }
+
 template <int BLOCK_N, int A_MODE, int B_MODE, int STAGES>
 __host__ __device__ constexpr int min_ctas() {
   // the accumulators (BLOCK_N fp32 registers per MMA thread) of a 256-thread gather CTA at
   // BLOCK_N = 128 do not fit the 128 registers a second CTA would leave
-  return (kthreads<A_MODE>() == 256 && BLOCK_N >= 128) ? 1
+  // halo kernels (128 threads): registers for four CTAs per SM, 128 per thread; their shared
+  // memory (B ring + two halos, 27-82 KB on the CIFAR shapes) decides how many actually fit
+  return A_MODE == A_HALO ? (BLOCK_N >= 128 ? 2 : 4)
+         : (kthreads<A_MODE>() == 256 && BLOCK_N >= 128) ? 1
          : ((2 * (STAGES * (A_BYTES + b_bytes<BLOCK_N, B_MODE>()) + 2048) <= 227 * 1024) ? 2 : 1);
 }
 
@@ -300,27 +358,37 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             const GemmParams p) {
   pdl_trigger();
   constexpr int B_BYTES = b_bytes<BLOCK_N, B_MODE>();
-  constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  constexpr int A_STAGE = a_stage_bytes<A_MODE>();
+  constexpr int STAGE_BYTES = A_STAGE + B_BYTES;
   constexpr bool A_GATHER = (A_MODE == A_GATHER_K || A_MODE == A_GATHER_MN);
+  constexpr bool HALO = (A_MODE == A_HALO);
   constexpr bool A_MN = (A_MODE == A_TMA_MN || A_MODE == A_GATHER_MN);
   constexpr bool B_MN = (B_MODE == B_TMA_MN);
   static_assert(!B_MN || BLOCK_N >= 64, "MN-major B tiles are built from 64-wide swizzle atoms");
-  static_assert(stage_f32_bytes<BLOCK_N>() <= STAGES * STAGE_BYTES, "epilogue staging exceeds the ring");
-  constexpr uint32_t TX_BYTES = (A_GATHER ? 0 : A_BYTES) + B_BYTES;
+  static_assert(HALO || stage_f32_bytes<BLOCK_N>() <= STAGES * STAGE_BYTES,
+                "epilogue staging exceeds the ring");
+  constexpr uint32_t TX_BYTES = (A_GATHER || HALO ? 0 : A_BYTES) + B_BYTES;
   constexpr int ACC = BLOCK_N / 2;                        // fp32 registers per 64-row half
   constexpr int SROW = BLOCK_N + 4;
 
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
+  __shared__ __align__(8) uint64_t halo_bar;
 
   // 1024-byte aligned tile area (SWIZZLE_128B atoms are 1024 B)
   uint8_t* tiles = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  // behind the ring: the gather lookup table (only as many entries as this geometry needs - a
-  // fixed-size table would cost the BLOCK_N = 64 conv kernels their second CTA per SM) and the
-  // tile's bias slice (the epilogue would otherwise wait on one L2 round trip per 8 columns)
-  int* const ktab = reinterpret_cast<int*>(tiles + (size_t)STAGES * STAGE_BYTES);
+  // halo kernels: the two blocks' halos follow the B ring; the epilogue's fp32 staging overlays
+  // ring and halos from the start of the tile area, and may be the larger of the two
+  uint8_t* const halo = tiles + (size_t)STAGES * STAGE_BYTES;
+  const int tile_area = HALO ? max(STAGES * STAGE_BYTES + 2 * p.hbytes, stage_f32_bytes<BLOCK_N>())
+                             : STAGES * STAGE_BYTES;
+  // behind the tile area: the gather lookup table (only as many entries as this geometry needs - a
+  // fixed-size table would cost the BLOCK_N = 64 conv kernels their second CTA per SM; halo
+  // kernels keep their per-k16-step descriptor offsets there) and the tile's bias slice (the
+  // epilogue would otherwise wait on one L2 round trip per 8 columns)
+  int* const ktab = reinterpret_cast<int*>(tiles + tile_area);
   float* const s_bias = reinterpret_cast<float*>(ktab + ((p.ktab_n + 3) & ~3));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -335,12 +403,34 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       mbar_init(&full_bar[s], (A_GATHER ? 128u : 0u) + 1u);
       mbar_init(&empty_bar[s], 1u);
     }
+    if (HALO) mbar_init(&halo_bar, 1u);
     fence_barrier_init();
     if (!A_GATHER) tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
   }
   if (A_GATHER) build_ktab(ktab, p.g, GKIND, p.gK);
+  if (HALO) build_halo_tab<GKIND>(ktab, p);
   pdl_wait();      // everything above overlapped the previous kernel's tail; global reads start here
+  if (HALO && threadIdx.x == 0) {
+    // the (8 + KY - 1) x (8 + KX - 1) window of each of the tile's two 8x8 blocks, one 8-channel
+    // plane per TMA box; out-of-image positions (padding, ragged edges, a block past the last
+    // image) arrive as zeros
+    const ConvGeomU& g = p.g;
+    const int nplanes = (GKIND == G_IM2COL ? g.C : g.F) / 8, plane = halo_plane_bytes(g);
+    mbar_arrive_expect_tx(&halo_bar, 2u * nplanes * (8 + g.KY - 1) * (8 + g.KX - 1) * 16);
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      const int b = blockIdx.y * 2 + h;
+      const int bx = b % p.hnbx, b2 = b / p.hnbx, by = b2 % p.hnby, n = b2 / p.hnby;
+      // fprop: output pixel (y, x) with tap (ky, kx) reads x[y + ky - PT][x + kx - PL];
+      // dgrad: input pixel (y, x) reads err_out[y + PT - ky][x + PL - kx]
+      const int x0 = GKIND == G_IM2COL ? bx * 8 - g.PL : bx * 8 + g.PL - (g.KX - 1);
+      const int y0 = GKIND == G_IM2COL ? by * 8 - g.PT : by * 8 + g.PT - (g.KY - 1);
+#pragma unroll 1
+      for (int c = 0; c < nplanes; ++c)
+        tma_load_4d(halo + h * p.hbytes + c * plane, &tmap_a, &halo_bar, c * 8, x0, y0, n);
+    }
+  }
   if (threadIdx.x < BLOCK_N) {
     const int n = blockIdx.x * BLOCK_N + threadIdx.x;
     s_bias[threadIdx.x] = (p.bias && n < p.N) ? __ldg(p.bias + n) : 0.f;
@@ -442,7 +532,7 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   auto issue_loads = [&](int i) {
     const int s = i % STAGES;
     uint8_t* sa = tiles + (size_t)s * STAGE_BYTES;
-    uint8_t* sb = sa + A_BYTES;
+    uint8_t* sb = sa + A_STAGE;
     const int k0 = (kb_begin + i) * BLOCK_K;
     mbar_arrive_expect_tx(&full_bar[s], TX_BYTES);
     if (A_MODE == A_IM2COL_K) {
@@ -483,23 +573,33 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   for (int j = 0; j < ACC; ++j) { acc0[j] = 0.f; acc1[j] = 0.f; }
   if (threadIdx.x == 0)
     for (int i = 0; i < STAGES && i < num_kb; ++i) issue_loads(i);
+  const uint32_t halo_sa = smem_u32(halo);
+  const uint32_t halo_sbo = (8 + p.g.KX - 1) * 16;       // one halo row = the next 8 tile rows
+  if (HALO) mbar_wait(&halo_bar, 0);
 #pragma unroll 1
   for (int i = 0; i < num_kb; ++i) {
     const int s = i % STAGES; const uint32_t ph = (i / STAGES) & 1;
     mbar_wait(&full_bar[s], ph);
     if (A_GATHER && GVEC == 2) fence_proxy_async_smem();   // LDGSTS data -> async proxy
     const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE_BYTES);
-    const uint32_t sb = sa + A_BYTES;
+    const uint32_t sb = sa + A_STAGE;
     wg_fence_regs(acc0); wg_fence_regs(acc1);
     wg_fence();
 #pragma unroll
     for (int k = 0; k < BLOCK_K / 16; ++k) {
       // K-major: 16 bf16 = 32 B along the swizzled row. MN-major: 16 k-rows = 2 atoms.
       // The 64-row halves of A are 8192 bytes apart in both layouts.
-      const uint64_t da0 = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024)
-                                : make_smem_desc(sa + k * 32, 16, 1024);
-      const uint64_t da1 = A_MN ? make_smem_desc(sa + 8192 + k * 2048, 8192, 1024)
-                                : make_smem_desc(sa + 8192 + k * 32, 16, 1024);
+      uint64_t da0, da1;
+      if (HALO) {
+        const uint32_t e = (uint32_t)ktab[(kb_begin + i) * (BLOCK_K / 16) + k];
+        const uint32_t a = halo_sa + (e & 0xFFFFu);
+        da0 = make_smem_desc_interleave(a, e >> 16, halo_sbo);
+        da1 = make_smem_desc_interleave(a + p.hbytes, e >> 16, halo_sbo);
+      } else {
+        da0 = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024) : make_smem_desc(sa + k * 32, 16, 1024);
+        da1 = A_MN ? make_smem_desc(sa + 8192 + k * 2048, 8192, 1024)
+                   : make_smem_desc(sa + 8192 + k * 32, 16, 1024);
+      }
       const uint64_t db = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024)
                                : make_smem_desc(sb + k * 32, 16, 1024);
       wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc0, da0, db, 1);
@@ -539,12 +639,13 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   named_bar_sync(1, 128);
   enum { EPI_BF16, EPI_RAW_T, EPI_RAW, EPI_SLOW, EPI_NONE, EPI_BIASROW, EPI_F32 };
   {
-    const int row = m0 + (int)threadIdx.x;
+    const int row = HALO ? halo_row<GKIND>(p, threadIdx.x) : m0 + (int)threadIdx.x;
     const bool raw32 = !p.out_bf16 && p.beta == 0.f && p.alpha == 1.f && !p.bias && p.act == 0;
     float* const rbase = reinterpret_cast<float*>(p.out) +
                          (p.split_stride > 0 ? (long long)blockIdx.z * p.split_stride : 0LL);
     int mode;
-    if (row >= p.M) mode = (p.bias_out && row == p.M) ? EPI_BIASROW : EPI_NONE;
+    if (row < 0) mode = EPI_NONE;
+    else if (row >= p.M) mode = (p.bias_out && row == p.M) ? EPI_BIASROW : EPI_NONE;
     else if (p.split_stride == 0 && !p.out_trans && p.out_bf16 && p.beta == 0.f) mode = EPI_BF16;
     else if (p.split_stride == 0 && !p.out_trans && !p.out_bf16 && p.beta == 0.f && !raw32)
       mode = EPI_F32;        // fp32 row-major with bias / activation (LSTM gate pre-activations,
@@ -744,12 +845,52 @@ static bool im2col_tma_enabled() {
   return on != 0;
 }
 
+// ---- A_HALO selection: a 4-D map over the NHWC source (x for fprop, err_out for dgrad) whose box
+// is one 8-channel plane of a block's halo, {8, 8 + KX - 1, 8 + KY - 1, 1}, no swizzle
+static long long g_halo_launches = 0;
+long long conv_halo_launches() { return g_halo_launches; }
+// ZNICZ_CONV_HALO=0 keeps the tap-mode LDGSTS gather for the shapes the halo kernel serves
+static bool conv_halo_enabled() {
+  static int on = -1;
+  if (on < 0) { const char* e = getenv("ZNICZ_CONV_HALO"); on = (e && atoi(e) == 0) ? 0 : 1; }
+  return on != 0;
+}
+// Tap-mode geometry (set_tap_mode) the halo kernel serves: unit stride, 8 / 16 / 32 inner channels
+// (tpk >= 2), a halo that fits HALO_MAX_BYTES. dgrad with 8 channels stays on the gather: its
+// flipped taps would need a negative LBO between the two taps of a k16 step.
+static bool halo_eligible(GemmParams& p, bool dgrad) {
+  const ConvGeomU& g = p.g;
+  if (!conv_halo_enabled() || g.SY != 1 || g.SX != 1 || g.tpk < 2 || (dgrad && g.tpk == 8)) return false;
+  if (8 + g.KX - 1 > 256 || 8 + g.KY - 1 > 256) return false;        // TMA box extent
+  p.hbytes = (g.inner / 8) * halo_plane_bytes(g);
+  if (p.hbytes > HALO_MAX_BYTES) return false;
+  const int PH = dgrad ? g.H : g.OH, PW = dgrad ? g.W : g.OW;
+  p.hnby = (PH + 7) / 8; p.hnbx = (PW + 7) / 8;
+  return (long long)g.N * p.hnby * p.hnbx < (1LL << 31);
+}
+static int make_map_halo(CUtensorMap* m, const void* ptr, int N, int H, int W, int C, int KY, int KX) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return -1;
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint32_t box[4] = {8u, (cuuint32_t)(8 + KX - 1), (cuuint32_t)(8 + KY - 1), 1u};
+  cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box,
+                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+
 template <int BN, int AM, int BM, int GK, int GV, int NS>
 static int launch_stages(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p_in, dim3 grid,
                          cudaStream_t st) {
-  constexpr int ring = NS * (A_BYTES + b_bytes<BN, BM>()) + 1024;
+  constexpr int ring = NS * (a_stage_bytes<AM>() + b_bytes<BN, BM>()) + 1024;
   constexpr bool gather = (AM == A_GATHER_K || AM == A_GATHER_MN);
-  constexpr int smem_max = ring + (gather ? KTAB * 4 : 0) + BN * 4 + 16;
+  constexpr bool halo = (AM == A_HALO);
+  // must match the kernel's tile area: halo kernels add two halos behind the ring, and their
+  // epilogue staging may need more than both
+  constexpr int area_max = halo ? std::max(ring + 2 * HALO_MAX_BYTES, stage_f32_bytes<BN>() + 1024) : ring;
+  constexpr int smem_max = area_max + (gather || halo ? KTAB * 4 : 0) + BN * 4 + 16;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_umma_k<BN, AM, BM, GK, GV, NS>,
@@ -763,7 +904,9 @@ static int launch_stages(const CUtensorMap& ta, const CUtensorMap& tb, const Gem
     const int step = p.g.vec ? 8 : 1;
     p.ktab_n = p.g.tpk > 0 ? p.g.ntaps : std::min(KTAB, (p.gK + step - 1) / step);
   }
-  const int smem = ring + ((p.ktab_n + 3) & ~3) * 4 + BN * 4;
+  if (halo) p.ktab_n = p.k_blocks_per_split * (BLOCK_K / 16);    // build_halo_tab(): one per k16 step
+  const int area = halo ? std::max(ring + 2 * p.hbytes, stage_f32_bytes<BN>() + 1024) : ring;
+  const int smem = area + ((p.ktab_n + 3) & ~3) * 4 + BN * 4;
   launch_k(gemm_umma_k<BN, AM, BM, GK, GV, NS>, grid, kthreads<AM>(), smem, st, ta, tb, p);
   return (int)cudaGetLastError();
 }
@@ -771,7 +914,8 @@ static int launch_stages(const CUtensorMap& ta, const CUtensorMap& tb, const Gem
 template <int BN, int AM, int BM, int GK, int GV>
 static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int splits,
                       cudaStream_t st) {
-  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  // halo kernels: one tile = two 8x8 pixel blocks, numbered over (image, block row, block column)
+  const int m_tiles = AM == A_HALO ? (p.g.N * p.hnby * p.hnbx + 1) / 2 : (p.M + BLOCK_M - 1) / BLOCK_M;
   dim3 grid((p.N + BN - 1) / BN, m_tiles, splits);
   // Short reductions (K <= 4 k-blocks, e.g. a 5x5 first layer on 8 padded channels) in grids of
   // several waves: a 3-stage ring already holds almost the whole K and is small enough for a
@@ -782,6 +926,12 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPa
     if (s3 < 0) { const char* e = getenv("ZNICZ_UMMA_S3"); s3 = e ? atoi(e) : 1; }
     if (s3 && p.k_blocks_per_split <= 4 && ctas > 2 * num_sms())
       return launch_stages<BN, AM, BM, GK, GV, 3>(ta, tb, p, grid, st);
+  }
+  // Halo kernels keep only B in the ring, and the MMAs of a k-block are a few hundred cycles: with
+  // 4 stages a 13-k-block reduction (5x5 x 32 channels) waits on ~3 serial refill round trips.
+  // 8 B stages halve that; short reductions keep 4 stages and their CTAs per SM.
+  if constexpr (AM == A_HALO) {
+    if (p.k_blocks_per_split > STAGES_DEFAULT) return launch_stages<BN, AM, BM, GK, GV, 8>(ta, tb, p, grid, st);
   }
   return launch_stages<BN, AM, BM, GK, GV, STAGES_DEFAULT>(ta, tb, p, grid, st);
 }
@@ -919,7 +1069,16 @@ int launch_conv_fprop_umma(const void* x, const void* w_lp, long long ldw, const
       return launch_bn<A_IM2COL_K, B_TMA_K, G_IM2COL, 0>(bn, ti, tb, p, 1, st);
     }
   }
-  if (set_tap_mode(p.g, C, false)) return launch_bn<A_GATHER_K, B_TMA_K, G_IM2COL, 2>(bn, ta, tb, p, 1, st);
+  if (set_tap_mode(p.g, C, false)) {
+    if (halo_eligible(p, false)) {
+      CUtensorMap th;
+      r = make_map_halo(&th, x, N, H, W, C, KY, KX);
+      if (r) return r;
+      ++g_halo_launches;
+      return launch_bn<A_HALO, B_TMA_K, G_IM2COL, 0>(bn, th, tb, p, 1, st);
+    }
+    return launch_bn<A_GATHER_K, B_TMA_K, G_IM2COL, 2>(bn, ta, tb, p, 1, st);
+  }
   if (C % 8 == 0) return launch_bn<A_GATHER_K, B_TMA_K, G_IM2COL, 1>(bn, ta, tb, p, 1, st);
   return launch_bn<A_GATHER_K, B_TMA_K, G_IM2COL, 0>(bn, ta, tb, p, 1, st);
 }
@@ -968,7 +1127,16 @@ int launch_conv_dgrad_umma(const void* err_out, const void* wd_lp, long long ldc
       return launch_bn<A_IM2COL_K, B_TMA_MN, G_DGRAD, 0>(bn, ti, tb, p, 1, st);
     }
   }
-  if (set_tap_mode(p.g, F, true)) return launch_bn<A_GATHER_K, B_TMA_MN, G_DGRAD, 2>(bn, ta, tb, p, 1, st);
+  if (set_tap_mode(p.g, F, true)) {
+    if (halo_eligible(p, true)) {
+      CUtensorMap th;
+      r = make_map_halo(&th, err_out, N, OH, OW, F, KY, KX);
+      if (r) return r;
+      ++g_halo_launches;
+      return launch_bn<A_HALO, B_TMA_MN, G_DGRAD, 0>(bn, th, tb, p, 1, st);
+    }
+    return launch_bn<A_GATHER_K, B_TMA_MN, G_DGRAD, 2>(bn, ta, tb, p, 1, st);
+  }
   if (F % 8 == 0) return launch_bn<A_GATHER_K, B_TMA_MN, G_DGRAD, 1>(bn, ta, tb, p, 1, st);
   return launch_bn<A_GATHER_K, B_TMA_MN, G_DGRAD, 0>(bn, ta, tb, p, 1, st);
 }
