@@ -18,8 +18,8 @@
 //
 // This covers: FC forward (TMA_K x TMA_K, fused bias+activation), FC dgrad (TMA_K x TMA_MN,
 // alpha/beta), FC wgrad (TMA_MN x TMA_MN), conv fprop (GATHER_K x TMA_K, fused bias+act),
-// conv dgrad (GATHER_K x TMA_MN, no atomics), conv wgrad (GATHER_MN x TMA_MN, split-K partials
-// that the fused update kernel sums in fixed order).
+// conv dgrad (GATHER_K x TMA_MN, no atomics), conv wgrad (GATHER_MN or HALO_MN x TMA_MN, split-K
+// partials that the fused update kernel sums in fixed order).
 #include "common.cuh"
 #include "umma.cuh"
 #include <stdlib.h>
@@ -39,7 +39,16 @@ using namespace umma;
 // bytes of a plane, SBO = one halo row. The tap-mode gather instead fetches each input byte once
 // per filter tap (25x for 5x5). The k16 steps issue the same products in the same order as the
 // gather, so the results are bit-identical.
-enum { A_TMA_K = 0, A_TMA_MN = 1, A_GATHER_K = 2, A_GATHER_MN = 3, A_IM2COL_K = 4, A_HALO = 5 };
+// A_HALO_MN: the conv weight gradient's im2col operand (M = kidx, K = pixels) for the same stride-1,
+// 8 / 16 / 32-channel geometries. A k-block (64 consecutive pixels = 64 / OW whole output rows, or
+// a 64-pixel row segment) needs one band of the input, (rows + KY - 1) x (cols + KX - 1) pixels,
+// loaded by TMA per 8-channel plane into each ring stage next to the err tile. The A operand is
+// MN-major without swizzle: a core matrix (8 pixels x 8 channels) is 128 contiguous bytes of a
+// plane, and the 8 core matrices along M of one m64 wgmma are the 8 kx slots of one (plane, ky)
+// "group", 16 bytes apart (slots >= KX read neighbouring pixels and are dropped). Every pixel
+// k16 step of the gather is issued unchanged, so the results are bit-identical to it.
+enum { A_TMA_K = 0, A_TMA_MN = 1, A_GATHER_K = 2, A_GATHER_MN = 3, A_IM2COL_K = 4, A_HALO = 5,
+       A_HALO_MN = 6 };
 enum { B_TMA_K = 0, B_TMA_MN = 1 };
 enum { G_NONE = 0, G_IM2COL = 1, G_DGRAD = 2 };
 
@@ -48,6 +57,8 @@ constexpr int BLOCK_K = 64;          // bf16 elements = 128 bytes = one SW128 ro
 constexpr int STAGES_DEFAULT = 4;   // 3 for short gather reductions: see launch_cfg
 constexpr int A_BYTES = BLOCK_M * 128;
 constexpr int HALO_MAX_BYTES = 32 * 1024;   // one block's halo (A_HALO), at most
+constexpr int BAND_MAX_BYTES = 16 * 1024;   // the planes of one ring stage's band (A_HALO_MN), at most
+constexpr int BAND_GROUPS = 3;              // A_HALO_MN: m64 groups (accumulator sets) per CTA
 
 struct ConvGeomU {
   int N, H, W, C, OH, OW, F, KY, KX, SY, SX, PT, PL;
@@ -76,7 +87,11 @@ struct GemmParams {
   int gK;                      // valid extent of the gathered K (fprop/dgrad) or M (wgrad) index
   int ktab_n;                  // entries of the gather lookup table (dynamic shared memory)
   // A_HALO: 8x8 pixel blocks per image row / column, and the bytes one block's halo occupies
+  // (A_HALO_MN: the bytes of one ring stage's band)
   int hnbx, hnby, hbytes;
+  // A_HALO_MN: band width / height in pixels, bytes per plane, (plane, ky) groups, and groups
+  // including the bias group (one more when bias_out is set)
+  int bw, bh, bplane, bgroups, bvgroups;
 };
 
 // ---- gather: 8 consecutive "inner" indices of one "pixel" -> 16 bytes ------------------------
@@ -324,6 +339,47 @@ __device__ __noinline__ void epi_store_slow(const GemmParams& p, int row, int n,
   }
 }
 
+// A_HALO_MN epilogue: the three groups' accumulators go through shared memory (stg, the idle ring)
+// as rows [group][slot][channel]; row (slot, channel) of group (plane, ky) is kidx
+// (ky * KX + slot) * C + plane * 8 + channel of partials[z][f][kidx], slots >= KX are dropped, and
+// row 0 of the bias group is bias_out[z][f]. Consecutive threads take consecutive rows, so that
+// a column's stores are runs of consecutive kidx. Empty splits store their zeros like the others.
+template <int BLOCK_N>
+__device__ __forceinline__ void band_epilogue(const GemmParams& p, float* stg, const float (&a0)[BLOCK_N / 2],
+                                              const float (&a1)[BLOCK_N / 2], const float (&a2)[BLOCK_N / 2]) {
+  constexpr int SROW = BLOCK_N + 4;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r0 = 16 * warp + (lane >> 2), cq = 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < BLOCK_N / 8; ++i) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int r = r0 + 8 * hh, c = 8 * i + cq, e = 4 * i + 2 * hh;
+      *reinterpret_cast<float2*>(stg + r * SROW + c) = make_float2(a0[e], a0[e + 1]);
+      *reinterpret_cast<float2*>(stg + (64 + r) * SROW + c) = make_float2(a1[e], a1[e + 1]);
+      *reinterpret_cast<float2*>(stg + (128 + r) * SROW + c) = make_float2(a2[e], a2[e + 1]);
+    }
+  }
+  named_bar_sync(1, 128);
+  const ConvGeomU& g = p.g;
+  const int n0 = blockIdx.x * BLOCK_N, ncols = min(BLOCK_N, p.N - n0);
+  float* const rbase = reinterpret_cast<float*>(p.out) + (long long)blockIdx.z * p.split_stride;
+#pragma unroll 1
+  for (int row = threadIdx.x; row < BAND_GROUPS * 64; row += 128) {
+    const int gv = blockIdx.y * BAND_GROUPS + (row >> 6), slot = (row >> 3) & 7, ch = row & 7;
+    const float* const srow = stg + row * SROW;
+    if (gv < p.bgroups) {
+      if (slot >= g.KX) continue;
+      const int pl = gv / g.KY, ky = gv - pl * g.KY;
+      float* const q = rbase + (long long)n0 * p.ldo + (ky * g.KX + slot) * g.C + pl * 8 + ch;
+#pragma unroll 4
+      for (int c = 0; c < ncols; ++c) q[(long long)c * p.ldo] = srow[c];
+    } else if (gv == p.bgroups && (row & 63) == 0 && p.bias_out) {
+      for (int c = 0; c < ncols; ++c) p.bias_out[(long long)blockIdx.z * p.N + n0 + c] = srow[c];
+    }
+  }
+}
+
 // Threads: warpgroup 0 (warps 0-3) issues the wgmma and runs the epilogue, its thread 0 also issues
 // the TMA loads; gather kernels add warpgroup 1 (warps 4-7) as the implicit-GEMM producers.
 template <int A_MODE>
@@ -337,9 +393,18 @@ __host__ __device__ constexpr int stage_f32_bytes() {
   return ((BLOCK_M * (BLOCK_N + 4) * 4) + 1023) & ~1023;
 }
 
-// bytes of one ring stage that hold A (the halo kernel keeps A outside the ring)
+// A_HALO_MN: the same staging for BAND_GROUPS x 64 rows
+template <int BLOCK_N>
+__host__ __device__ constexpr int band_f32_bytes() {
+  return ((BAND_GROUPS * 64 * (BLOCK_N + 4) * 4) + 1023) & ~1023;
+}
+
+// bytes of one ring stage that hold A (the halo kernels keep A outside the constexpr ring: A_HALO
+// in two halos, A_HALO_MN in a second ring of bands whose stage size is known at launch)
 template <int A_MODE>
-__host__ __device__ constexpr int a_stage_bytes() { return A_MODE == A_HALO ? 0 : A_BYTES; }
+__host__ __device__ constexpr int a_stage_bytes() {
+  return (A_MODE == A_HALO || A_MODE == A_HALO_MN) ? 0 : A_BYTES;
+}
 
 template <int BLOCK_N, int A_MODE, int B_MODE, int STAGES>
 __host__ __device__ constexpr int min_ctas() {
@@ -347,7 +412,9 @@ __host__ __device__ constexpr int min_ctas() {
   // BLOCK_N = 128 do not fit the 128 registers a second CTA would leave
   // halo kernels (128 threads): registers for four CTAs per SM, 128 per thread; their shared
   // memory (B ring + two halos, 27-82 KB on the CIFAR shapes) decides how many actually fit
-  return A_MODE == A_HALO ? (BLOCK_N >= 128 ? 2 : 4)
+  // band kernels: BAND_GROUPS x BLOCK_N / 2 accumulators per thread, two CTAs per SM
+  return A_MODE == A_HALO_MN ? 2
+         : A_MODE == A_HALO ? (BLOCK_N >= 128 ? 2 : 4)
          : (kthreads<A_MODE>() == 256 && BLOCK_N >= 128) ? 1
          : ((2 * (STAGES * (A_BYTES + b_bytes<BLOCK_N, B_MODE>()) + 2048) <= 227 * 1024) ? 2 : 1);
 }
@@ -362,12 +429,14 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   constexpr int STAGE_BYTES = A_STAGE + B_BYTES;
   constexpr bool A_GATHER = (A_MODE == A_GATHER_K || A_MODE == A_GATHER_MN);
   constexpr bool HALO = (A_MODE == A_HALO);
-  constexpr bool A_MN = (A_MODE == A_TMA_MN || A_MODE == A_GATHER_MN);
+  constexpr bool BAND = (A_MODE == A_HALO_MN);
+  constexpr bool A_MN = (A_MODE == A_TMA_MN || A_MODE == A_GATHER_MN || BAND);
   constexpr bool B_MN = (B_MODE == B_TMA_MN);
   static_assert(!B_MN || BLOCK_N >= 64, "MN-major B tiles are built from 64-wide swizzle atoms");
-  static_assert(HALO || stage_f32_bytes<BLOCK_N>() <= STAGES * STAGE_BYTES,
+  static_assert(HALO || BAND || stage_f32_bytes<BLOCK_N>() <= STAGES * STAGE_BYTES,
                 "epilogue staging exceeds the ring");
-  constexpr uint32_t TX_BYTES = (A_GATHER || HALO ? 0 : A_BYTES) + B_BYTES;
+  static_assert(!BAND || (B_MN && GKIND == G_IM2COL), "A_HALO_MN is the conv wgrad operand");
+  constexpr uint32_t TX_BYTES = (A_GATHER || HALO || BAND ? 0 : A_BYTES) + B_BYTES;
   constexpr int ACC = BLOCK_N / 2;                        // fp32 registers per 64-row half
   constexpr int SROW = BLOCK_N + 4;
 
@@ -381,9 +450,12 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   // halo kernels: the two blocks' halos follow the B ring; the epilogue's fp32 staging overlays
   // ring and halos from the start of the tile area, and may be the larger of the two
+  // band kernels: the ring of bands (STAGES x hbytes) follows the B ring, then the 128-byte block
+  // of bias "ones" rows; their staging is band_f32_bytes
   uint8_t* const halo = tiles + (size_t)STAGES * STAGE_BYTES;
   const int tile_area = HALO ? max(STAGES * STAGE_BYTES + 2 * p.hbytes, stage_f32_bytes<BLOCK_N>())
-                             : STAGES * STAGE_BYTES;
+                        : BAND ? max(STAGES * (STAGE_BYTES + p.hbytes) + 128, band_f32_bytes<BLOCK_N>())
+                               : STAGES * STAGE_BYTES;
   // behind the tile area: the gather lookup table (only as many entries as this geometry needs - a
   // fixed-size table would cost the BLOCK_N = 64 conv kernels their second CTA per SM; halo
   // kernels keep their per-k16-step descriptor offsets there) and the tile's bias slice (the
@@ -410,6 +482,21 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   }
   if (A_GATHER) build_ktab(ktab, p.g, GKIND, p.gK);
   if (HALO) build_halo_tab<GKIND>(ktab, p);
+  // band kernels: group j of this CTA is gv = blockIdx.y * BAND_GROUPS + j, numbered plane-major
+  // (gv = plane * KY + ky) so that a CTA loads as few planes as possible; gv == bgroups is the bias
+  // group, whose A is the ones block: 8 rows of {1, 0, ..., 0} read with LBO = SBO = 0, so that
+  // product row 0 of the group is sum_pixels err[pixel][f], the gather's ones row
+  int band_plo = 0, band_np = 0;
+  uint8_t* const ones = halo + (size_t)STAGES * p.hbytes;
+  if (BAND) {
+    const int g0 = blockIdx.y * BAND_GROUPS, gl = min(g0 + BAND_GROUPS, p.bgroups) - 1;
+    band_plo = g0 / p.g.KY;
+    band_np = gl >= g0 ? gl / p.g.KY - band_plo + 1 : 0;
+    if (threadIdx.x < 64)
+      reinterpret_cast<__nv_bfloat16*>(ones)[threadIdx.x] =
+          __float2bfloat16_rn((threadIdx.x & 7) == 0 ? 1.f : 0.f);
+    fence_proxy_async_smem();
+  }
   pdl_wait();      // everything above overlapped the previous kernel's tail; global reads start here
   if (HALO && threadIdx.x == 0) {
     // the (8 + KY - 1) x (8 + KX - 1) window of each of the tile's two 8x8 blocks, one 8-channel
@@ -534,8 +621,19 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     uint8_t* sa = tiles + (size_t)s * STAGE_BYTES;
     uint8_t* sb = sa + A_STAGE;
     const int k0 = (kb_begin + i) * BLOCK_K;
-    mbar_arrive_expect_tx(&full_bar[s], TX_BYTES);
-    if (A_MODE == A_IM2COL_K) {
+    mbar_arrive_expect_tx(&full_bar[s], TX_BYTES + (BAND ? band_np * p.bw * p.bh * 16 : 0));
+    if (BAND) {
+      // the band of pixels k0 .. k0 + 63 (one image: (OH * OW) % 64 == 0), one box per plane;
+      // output pixel (oy, ox) with tap (ky, kx) reads x[oy + ky - PT][ox + kx - PL]
+      const ConvGeomU& g = p.g;
+      const int img = g.OH * g.OW, n = k0 / img, rem = k0 - n * img, oy = rem / g.OW;
+      const int ox = rem - oy * g.OW;
+      uint8_t* const band = halo + (size_t)s * p.hbytes;
+#pragma unroll 1
+      for (int j = 0; j < band_np; ++j)
+        tma_load_4d(band + j * p.bplane, &tmap_a, &full_bar[s], (band_plo + j) * 8, ox - g.PL,
+                    oy - g.PT, n);
+    } else if (A_MODE == A_IM2COL_K) {
       // conv fprop / stride-1 dgrad: tile rows = pixels m0 .. m0 + 127, k-block = 64
       // channels of ONE filter tap
       const ConvGeomU& g = p.g;
@@ -569,13 +667,38 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   };
 
   float acc0[ACC], acc1[ACC];                 // rows 0-63 / 64-127 of the tile
+  float acc2[BAND ? ACC : 1];                 // band kernels: the third group
 #pragma unroll
   for (int j = 0; j < ACC; ++j) { acc0[j] = 0.f; acc1[j] = 0.f; }
+#pragma unroll
+  for (int j = 0; j < (BAND ? ACC : 1); ++j) acc2[j] = 0.f;
   if (threadIdx.x == 0)
     for (int i = 0; i < STAGES && i < num_kb; ++i) issue_loads(i);
   const uint32_t halo_sa = smem_u32(halo);
   const uint32_t halo_sbo = (8 + p.g.KX - 1) * 16;       // one halo row = the next 8 tile rows
   if (HALO) mbar_wait(&halo_bar, 0);
+  // band kernels: byte offset of each group's slot-0 core matrix for pixel 0 (ones: the group
+  // reads the ones block), of each k16 step's first pixel, and between its two 8-pixel halves
+  // (the next 8 pixels of the row, or the next band row when OW = 8)
+  uint32_t band_goff[BAND_GROUPS], band_soff[BLOCK_K / 16], band_kstr = 0;
+  bool band_one[BAND_GROUPS];
+  if (BAND) {
+    const ConvGeomU& g = p.g;
+    const int owb = min(g.OW, 64);
+#pragma unroll
+    for (int j = 0; j < BAND_GROUPS; ++j) {
+      const int gv = blockIdx.y * BAND_GROUPS + j, pl = gv / g.KY, ky = gv - pl * g.KY;
+      band_one[j] = gv >= p.bgroups;
+      band_goff[j] = band_one[j] ? 0u : (uint32_t)((pl - band_plo) * p.bplane + ky * p.bw * 16);
+    }
+#pragma unroll
+    for (int k = 0; k < BLOCK_K / 16; ++k) {
+      const int r = (16 * k) / owb, c = 16 * k - r * owb;
+      band_soff[k] = (uint32_t)((r * p.bw + c) * 16);
+    }
+    band_kstr = owb == 8 ? p.bw * 16 : 128;
+  }
+  const uint64_t ones_desc = make_smem_desc_interleave(smem_u32(ones), 0, 0);
 #pragma unroll 1
   for (int i = 0; i < num_kb; ++i) {
     const int s = i % STAGES; const uint32_t ph = (i / STAGES) & 1;
@@ -583,14 +706,25 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     if (A_GATHER && GVEC == 2) fence_proxy_async_smem();   // LDGSTS data -> async proxy
     const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE_BYTES);
     const uint32_t sb = sa + A_STAGE;
+    const uint32_t band = halo_sa + s * p.hbytes;
     wg_fence_regs(acc0); wg_fence_regs(acc1);
+    if (BAND) wg_fence_regs(acc2);
     wg_fence();
 #pragma unroll
     for (int k = 0; k < BLOCK_K / 16; ++k) {
       // K-major: 16 bf16 = 32 B along the swizzled row. MN-major: 16 k-rows = 2 atoms.
       // The 64-row halves of A are 8192 bytes apart in both layouts.
-      uint64_t da0, da1;
-      if (HALO) {
+      uint64_t da0, da1, da2 = 0;
+      if (BAND) {
+        // MN-major, no swizzle: SBO = 16 bytes between the kx slots along M, LBO between the two
+        // 8-pixel halves along K
+        uint64_t d[BAND_GROUPS];
+#pragma unroll
+        for (int j = 0; j < BAND_GROUPS; ++j)
+          d[j] = band_one[j] ? ones_desc
+                             : make_smem_desc_interleave(band + band_goff[j] + band_soff[k], band_kstr, 16);
+        da0 = d[0]; da1 = d[1]; da2 = d[2];
+      } else if (HALO) {
         const uint32_t e = (uint32_t)ktab[(kb_begin + i) * (BLOCK_K / 16) + k];
         const uint32_t a = halo_sa + (e & 0xFFFFu);
         da0 = make_smem_desc_interleave(a, e >> 16, halo_sbo);
@@ -604,9 +738,11 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                                : make_smem_desc(sb + k * 32, 16, 1024);
       wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc0, da0, db, 1);
       wgmma_bf16<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc1, da1, db, 1);
+      if constexpr (BAND) wgmma_bf16<BLOCK_N, 1, 1>(acc2, da2, db, 1);
     }
     wg_commit();
     wg_fence_regs(acc0); wg_fence_regs(acc1);
+    if (BAND) wg_fence_regs(acc2);
     wg_wait<1>();                               // the MMAs of k-block i - 1 have retired
     if (i > 0 && threadIdx.x == 0) {
       const int sp = (i - 1) % STAGES;
@@ -616,6 +752,11 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   }
   wg_wait<0>();
   wg_fence_regs(acc0); wg_fence_regs(acc1);
+  if constexpr (BAND) {
+    wg_fence_regs(acc2);
+    band_epilogue<BLOCK_N>(p, reinterpret_cast<float*>(tiles), acc0, acc1, acc2);
+    return;
+  }
 
   // ===================== epilogue =====================
   // The accumulator fragments go through shared memory (the ring is idle: every k-block has been
@@ -868,12 +1009,37 @@ static bool halo_eligible(GemmParams& p, bool dgrad) {
   p.hnby = (PH + 7) / 8; p.hnbx = (PW + 7) / 8;
   return (long long)g.N * p.hnby * p.hnbx < (1LL << 31);
 }
-static int make_map_halo(CUtensorMap* m, const void* ptr, int N, int H, int W, int C, int KY, int KX) {
+// The conv weight gradient (A_HALO_MN) of the same tap-mode geometries, with F <= 64 (one BLOCK_N
+// = 64 tile: three groups of accumulators fit the registers), KX <= 8 (one group's 8 kx slots),
+// k-blocks of whole output rows (OW = 8 / 16 / 32 / 64) or 64-pixel row segments (OW % 64 == 0)
+// that never straddle two images, and a band that fits BAND_MAX_BYTES per stage. Fills the band
+// fields of p; the group count includes the bias group when p.bias_out is set.
+static bool band_eligible(GemmParams& p) {
+  const ConvGeomU& g = p.g;
+  if (!conv_halo_enabled() || g.SY != 1 || g.SX != 1 || g.tpk < 2 || g.F > 64 || g.KX > 8) return false;
+  const bool rows = g.OW % 8 == 0 && 64 % g.OW == 0;
+  if ((!rows && g.OW % 64) || (g.OH * g.OW) % 64) return false;
+  p.bw = (rows ? g.OW : 64) + g.KX - 1;
+  p.bh = (rows ? 64 / g.OW : 1) + g.KY - 1;
+  if (p.bw > 256 || p.bh > 256) return false;                       // TMA box extent
+  p.bplane = (p.bw * p.bh * 16 + 127) & ~127;
+  p.bgroups = g.KY * (g.C / 8);
+  p.bvgroups = p.bgroups + (p.bias_out ? 1 : 0);
+  int np = 0;                  // planes of the widest CTA (groups are numbered plane * KY + ky)
+  for (int g0 = 0; g0 < p.bgroups; g0 += BAND_GROUPS)
+    np = std::max(np, (std::min(g0 + BAND_GROUPS, p.bgroups) - 1) / g.KY - g0 / g.KY + 1);
+  // slots >= KX of the last pixels read up to (8 - KX) * 16 bytes past the last plane
+  p.hbytes = np * p.bplane + 128;
+  return p.hbytes <= BAND_MAX_BYTES;
+}
+static int make_map_halo(CUtensorMap* m, const void* ptr, int N, int H, int W, int C, int KY, int KX,
+                         int box_w = 0, int box_h = 0) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return -1;
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
   cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {8u, (cuuint32_t)(8 + KX - 1), (cuuint32_t)(8 + KY - 1), 1u};
+  // box {8 channels, 8 + KX - 1, 8 + KY - 1, 1} (A_HALO) or {8, box_w, box_h, 1} (a band)
+  cuuint32_t box[4] = {8u, (cuuint32_t)(box_w ? box_w : 8 + KX - 1), (cuuint32_t)(box_h ? box_h : 8 + KY - 1), 1u};
   cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box,
                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
@@ -887,9 +1053,12 @@ static int launch_stages(const CUtensorMap& ta, const CUtensorMap& tb, const Gem
   constexpr int ring = NS * (a_stage_bytes<AM>() + b_bytes<BN, BM>()) + 1024;
   constexpr bool gather = (AM == A_GATHER_K || AM == A_GATHER_MN);
   constexpr bool halo = (AM == A_HALO);
-  // must match the kernel's tile area: halo kernels add two halos behind the ring, and their
-  // epilogue staging may need more than both
-  constexpr int area_max = halo ? std::max(ring + 2 * HALO_MAX_BYTES, stage_f32_bytes<BN>() + 1024) : ring;
+  constexpr bool band = (AM == A_HALO_MN);
+  // must match the kernel's tile area: halo kernels add two halos behind the ring, band kernels a
+  // ring of bands and the ones block; the epilogue staging of both may need more
+  constexpr int area_max = halo ? std::max(ring + 2 * HALO_MAX_BYTES, stage_f32_bytes<BN>() + 1024)
+                           : band ? std::max(ring + NS * BAND_MAX_BYTES + 128, band_f32_bytes<BN>() + 1024)
+                                  : ring;
   constexpr int smem_max = area_max + (gather || halo ? KTAB * 4 : 0) + BN * 4 + 16;
   static bool attr_set = false;
   if (!attr_set) {
@@ -905,7 +1074,9 @@ static int launch_stages(const CUtensorMap& ta, const CUtensorMap& tb, const Gem
     p.ktab_n = p.g.tpk > 0 ? p.g.ntaps : std::min(KTAB, (p.gK + step - 1) / step);
   }
   if (halo) p.ktab_n = p.k_blocks_per_split * (BLOCK_K / 16);    // build_halo_tab(): one per k16 step
-  const int area = halo ? std::max(ring + 2 * p.hbytes, stage_f32_bytes<BN>() + 1024) : ring;
+  const int area = halo ? std::max(ring + 2 * p.hbytes, stage_f32_bytes<BN>() + 1024)
+                   : band ? std::max(ring + NS * p.hbytes + 128, band_f32_bytes<BN>() + 1024)
+                          : ring;
   const int smem = area + ((p.ktab_n + 3) & ~3) * 4 + BN * 4;
   launch_k(gemm_umma_k<BN, AM, BM, GK, GV, NS>, grid, kthreads<AM>(), smem, st, ta, tb, p);
   return (int)cudaGetLastError();
@@ -915,7 +1086,10 @@ template <int BN, int AM, int BM, int GK, int GV>
 static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int splits,
                       cudaStream_t st) {
   // halo kernels: one tile = two 8x8 pixel blocks, numbered over (image, block row, block column)
-  const int m_tiles = AM == A_HALO ? (p.g.N * p.hnby * p.hnbx + 1) / 2 : (p.M + BLOCK_M - 1) / BLOCK_M;
+  // band kernels: BAND_GROUPS (plane, ky) groups per CTA
+  const int m_tiles = AM == A_HALO ? (p.g.N * p.hnby * p.hnbx + 1) / 2
+                      : AM == A_HALO_MN ? (p.bvgroups + BAND_GROUPS - 1) / BAND_GROUPS
+                                        : (p.M + BLOCK_M - 1) / BLOCK_M;
   dim3 grid((p.N + BN - 1) / BN, m_tiles, splits);
   // Short reductions (K <= 4 k-blocks, e.g. a 5x5 first layer on 8 padded channels) in grids of
   // several waves: a 3-stage ring already holds almost the whole K and is small enough for a
@@ -930,7 +1104,8 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const GemmPa
   // Halo kernels keep only B in the ring, and the MMAs of a k-block are a few hundred cycles: with
   // 4 stages a 13-k-block reduction (5x5 x 32 channels) waits on ~3 serial refill round trips.
   // 8 B stages halve that; short reductions keep 4 stages and their CTAs per SM.
-  if constexpr (AM == A_HALO) {
+  // Band kernels likewise: an 8-stage ring of err tiles and bands for reductions longer than 4.
+  if constexpr (AM == A_HALO || AM == A_HALO_MN) {
     if (p.k_blocks_per_split > STAGES_DEFAULT) return launch_stages<BN, AM, BM, GK, GV, 8>(ta, tb, p, grid, st);
   }
   return launch_stages<BN, AM, BM, GK, GV, STAGES_DEFAULT>(ta, tb, p, grid, st);
@@ -1180,6 +1355,16 @@ int launch_conv_wgrad_umma(const void* err_out, const void* x, float* partials, 
       if (!ones && cudaGetSymbolAddress(&ones, zn_ones_bf16) != cudaSuccess) ones = nullptr;
       row = ones != nullptr;
       if (row) { p.g.ones = (const __nv_bfloat16*)ones; p.bias_out = bias_parts; }
+    }
+    if (bn == 64 && band_eligible(p)) {
+      // the same products in the same pixel order as the gather below (and the bias row exactly
+      // where it would have one), from one band of x per k-block instead of a gather per tap
+      CUtensorMap th;
+      r = make_map_halo(&th, x, N, H, W, C, KY, KX, p.bw, p.bh);
+      if (r) return r;
+      ++g_halo_launches;
+      r = launch_cfg<64, A_HALO_MN, B_TMA_MN, G_IM2COL, 0>(th, tb, p, splits, st);
+      return (r == 0 && row) ? 1 : r;
     }
     r = launch_bn<A_GATHER_MN, B_TMA_MN, G_IM2COL, 2>(bn, ta, tb, p, splits, st);
     return (r == 0 && row) ? 1 : r;

@@ -259,6 +259,10 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t 
 // The same descriptor without swizzle (layout = 0, "interleave"), K-major: a core matrix is 8 rows
 // of 16 contiguous bytes (128 bytes); LBO = byte offset to the core matrix holding the next 8
 // elements along K, SBO = byte offset to the core matrix holding the next 8 rows.
+// MN-major (transposed operand) keeps the same roles: a core matrix is 8 k-rows of 8 contiguous
+// M / N elements, LBO = offset to the next 8 k-rows, SBO = offset to the next 8 M / N elements
+// (unlike the swizzled MN-major layouts above, where LBO steps along M / N). Checked on an H100
+// with a single m64n16k16 wgmma against both assignments.
 __device__ __forceinline__ uint64_t make_smem_desc_interleave(uint32_t smem_addr, uint32_t lbo_bytes,
                                                               uint32_t sbo_bytes) {
   uint64_t d = 0;
