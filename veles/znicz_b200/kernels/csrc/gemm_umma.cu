@@ -301,15 +301,35 @@ __device__ __forceinline__ void build_halo_tab(int* tab, const GemmParams& p) {
     tab[s] = (lbo << 16) | a;
   }
 }
-// GEMM row (output pixel; dgrad: input pixel) of tile row t, or -1 outside the image
+// GEMM row (output pixel; dgrad: input pixel) of row r of 8x8 block b, or -1 outside the image
 template <int KIND>
-__device__ __forceinline__ int halo_row(const GemmParams& p, int t) {
+__device__ __forceinline__ int halo_row(const GemmParams& p, int b, int r) {
   const ConvGeomU& g = p.g;
-  const int b = blockIdx.y * 2 + (t >> 6), r = t & 63;
   const int bx = b % p.hnbx, b2 = b / p.hnbx, by = b2 % p.hnby, n = b2 / p.hnby;
   const int PH = KIND == G_IM2COL ? g.OH : g.H, PW = KIND == G_IM2COL ? g.OW : g.W;
   const int y = by * 8 + (r >> 3), x = bx * 8 + (r & 7);
   return (n < g.N && y < PH && x < PW) ? (n * PH + y) * PW + x : -1;
+}
+// TMA loads of block b's (8 + KY - 1) x (8 + KX - 1) input window into dst, one 8-channel plane
+// per box, completing on bar (the caller arms it with halo_tx_bytes); out-of-image positions
+// (padding, ragged edges, a block past the last image) arrive as zeros
+template <int KIND>
+__device__ __forceinline__ void load_halo(uint8_t* dst, const CUtensorMap* tmap, uint64_t* bar,
+                                          const GemmParams& p, int b) {
+  const ConvGeomU& g = p.g;
+  const int nplanes = (KIND == G_IM2COL ? g.C : g.F) / 8, plane = halo_plane_bytes(g);
+  const int bx = b % p.hnbx, b2 = b / p.hnbx, by = b2 % p.hnby, n = b2 / p.hnby;
+  // fprop: output pixel (y, x) with tap (ky, kx) reads x[y + ky - PT][x + kx - PL];
+  // dgrad: input pixel (y, x) reads err_out[y + PT - ky][x + PL - kx]
+  const int x0 = KIND == G_IM2COL ? bx * 8 - g.PL : bx * 8 + g.PL - (g.KX - 1);
+  const int y0 = KIND == G_IM2COL ? by * 8 - g.PT : by * 8 + g.PT - (g.KY - 1);
+#pragma unroll 1
+  for (int c = 0; c < nplanes; ++c) tma_load_4d(dst + c * plane, tmap, bar, c * 8, x0, y0, n);
+}
+template <int KIND>
+__device__ __forceinline__ uint32_t halo_tx_bytes(const GemmParams& p) {
+  const ConvGeomU& g = p.g;
+  return (uint32_t)((KIND == G_IM2COL ? g.C : g.F) / 8) * (8 + g.KY - 1) * (8 + g.KX - 1) * 16;
 }
 
 template <int BLOCK_N, int B_MODE>
@@ -377,6 +397,159 @@ __device__ __forceinline__ void band_epilogue(const GemmParams& p, float* stg, c
     } else if (gv == p.bgroups && (row & 63) == 0 && p.bias_out) {
       for (int c = 0; c < ncols; ++c) p.bias_out[(long long)blockIdx.z * p.N + n0 + c] = srow[c];
     }
+  }
+}
+
+// The accumulator fragment of one m64 wgmma (warpgroup thread t = threadIdx.x % 128) -> rows
+// row0 .. row0 + 63 of the fp32 staging [rows][BLOCK_N + 4] (the pad makes the row reads of 8
+// consecutive threads hit distinct banks)
+template <int BLOCK_N>
+__device__ __forceinline__ void stage_acc(float* stg, int row0, const float (&acc)[BLOCK_N / 2]) {
+  constexpr int SROW = BLOCK_N + 4;
+  const int t = threadIdx.x & 127, r0 = row0 + 16 * (t >> 5) + ((t & 31) >> 2), cq = 2 * (t & 3);
+#pragma unroll
+  for (int i = 0; i < BLOCK_N / 8; ++i) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+      *reinterpret_cast<float2*>(stg + (r0 + 8 * hh) * SROW + 8 * i + cq) =
+          make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
+  }
+}
+
+// The epilogue of one GEMM row (row < 0: outside the image, nothing is stored): columns
+// n0 + c_lo .. n0 + c_hi - 1 (c_lo, c_hi multiples of 8) of the fp32 staging row srow, with the
+// tile's bias slice s_bias (indexed from n0); z is the split (fp32 partials, wgrad bias row).
+// A rolled loop over 8-column chunks (it runs once per tile, so every instruction of it is an
+// instruction-cache miss: a short loop body fetched once beats an unrolled one), output mode
+// decided once. SLOW = false compiles out the out-of-line epi_store_slow call, for callers that
+// never need it (bf16 row-major output without beta): a call inside a loop that issues wgmma makes
+// ptxas serialise the wgmma.
+template <bool SLOW = true>
+__device__ __forceinline__ void epilogue_row(const GemmParams& p, int row, const float* srow,
+                                             const float* s_bias, int n0, int c_lo, int c_hi, int z) {
+  enum { EPI_BF16, EPI_RAW_T, EPI_RAW, EPI_SLOW, EPI_NONE, EPI_BIASROW, EPI_F32 };
+  const bool raw32 = !p.out_bf16 && p.beta == 0.f && p.alpha == 1.f && !p.bias && p.act == 0;
+  float* const rbase = reinterpret_cast<float*>(p.out) +
+                       (p.split_stride > 0 ? (long long)z * p.split_stride : 0LL);
+  int mode;
+  if (row < 0) mode = EPI_NONE;
+  else if (row >= p.M) mode = (p.bias_out && row == p.M) ? EPI_BIASROW : EPI_NONE;
+  else if (p.split_stride == 0 && !p.out_trans && p.out_bf16 && p.beta == 0.f) mode = EPI_BF16;
+  else if (p.split_stride == 0 && !p.out_trans && !p.out_bf16 && p.beta == 0.f && !raw32)
+    mode = EPI_F32;        // fp32 row-major with bias / activation (LSTM gate pre-activations,
+                           // softmax logits): same inline path as bf16, fp32 stores
+  else if (raw32 && p.out_trans) mode = EPI_RAW_T;
+  else if (raw32 && (p.ldo & 3) == 0 && (reinterpret_cast<uintptr_t>(rbase) & 15) == 0)
+    mode = EPI_RAW;
+  else mode = EPI_SLOW;
+
+  auto emit = [&](const uint32_t (&r)[8], int c0) {
+    const int nb = n0 + c0;
+    if (mode == EPI_NONE) return;
+    if (mode == EPI_BIASROW) {       // product row M = column sums of err (see ConvGeomU::ones)
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (nb + j < p.N) p.bias_out[(long long)z * p.N + nb + j] = __uint_as_float(r[j]);
+      return;
+    }
+    if (mode == EPI_BF16 || mode == EPI_F32) {
+      float v[8];
+      {
+        const float4 b0 = *reinterpret_cast<const float4*>(s_bias + c0);
+        const float4 b1 = *reinterpret_cast<const float4*>(s_bias + c0 + 4);
+        v[0] = b0.x; v[1] = b0.y; v[2] = b0.z; v[3] = b0.w;
+        v[4] = b1.x; v[5] = b1.y; v[6] = b1.z; v[7] = b1.w;
+      }
+      // activation selected once per chunk (not per element): the executed path stays short
+      switch (p.act) {
+        // out = act(alpha * acc + bias): alpha is the err_input_alpha of dgrad (no bias,
+        // linear); every other caller passes alpha = 1
+        case ACT_LINEAR:
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[j] = fmaf(__uint_as_float(r[j]), p.alpha, v[j]);
+          break;
+        case ACT_STRICT_RELU:
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[j] = fmaxf(fmaf(__uint_as_float(r[j]), p.alpha, v[j]), 0.f);
+          break;
+        case ACT_TANH:
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            v[j] = 1.7159f * tanh_approx(0.6666f * fmaf(__uint_as_float(r[j]), p.alpha, v[j]));
+          break;
+        default:
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            v[j] = act_fwd5_fast(p.act, fmaf(__uint_as_float(r[j]), p.alpha, v[j]));
+      }
+      if (p.dmul != nullptr && mode == EPI_BF16) {
+        // err_input *= f'(x): x has the layout of the output (row pitch ldo)
+        const __nv_bfloat16* dx = p.dmul + (long long)row * p.ldo + nb;
+        if (nb + 8 <= p.N && (p.ldo & 7) == 0) {
+          float xv[8];
+          ld8(dx, xv);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[j] *= act_deriv(p.dact, 0.f, xv[j]);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (nb + j < p.N) v[j] *= act_deriv(p.dact, 0.f, __bfloat162float(dx[j]));
+        }
+      }
+      if (mode == EPI_F32) {
+        float* qf = reinterpret_cast<float*>(p.out) + (long long)row * p.ldo + nb;
+        if (nb + 8 <= p.N && (p.ldo & 3) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
+          reinterpret_cast<float4*>(qf)[0] = make_float4(v[0], v[1], v[2], v[3]);
+          reinterpret_cast<float4*>(qf)[1] = make_float4(v[4], v[5], v[6], v[7]);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (nb + j < p.N) qf[j] = v[j];
+        }
+        return;
+      }
+      __nv_bfloat16* q = reinterpret_cast<__nv_bfloat16*>(p.out) + (long long)row * p.ldo + nb;
+      if (nb + 8 <= p.N && (p.ldo & 7) == 0) {
+        st8(q, v);                   // bf16 pack: one 16-byte store per 8 outputs
+      } else {                       // ragged last chunk / row pitch not a multiple of 16 bytes
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (nb + j < p.N) q[j] = __float2bfloat16_rn(v[j]);
+      }
+    } else if (mode == EPI_RAW_T) {
+      // raw fp32 (split-K partials / FC weight gradients), transposed: for a fixed column the
+      // 32 lanes hold consecutive rows = one coalesced 128-byte store per column
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (nb + j < p.N) rbase[(long long)(nb + j) * p.ldo + row] = __uint_as_float(r[j]);
+    } else if (mode == EPI_RAW && nb + 8 <= p.N) {
+      float4* q = reinterpret_cast<float4*>(rbase + (long long)row * p.ldo + nb);
+      q[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]),
+                         __uint_as_float(r[3]));
+      q[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]),
+                         __uint_as_float(r[7]));
+    } else if (raw32) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (nb + j < p.N) rbase[(long long)row * p.ldo + nb + j] = __uint_as_float(r[j]);
+    } else if (SLOW) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)     // (static indices: r stays in registers)
+        if (nb + j < p.N) epi_store_slow(p, row, nb + j, __uint_as_float(r[j]), z);
+    }
+  };
+
+#pragma unroll 1
+  for (int c0 = c_lo; c0 < c_hi; c0 += 8) {
+    if (n0 + c0 >= p.N) break;     // chunk beyond the last column
+    uint32_t ra[8];
+    const float4 x0 = *reinterpret_cast<const float4*>(srow + c0);
+    const float4 x1 = *reinterpret_cast<const float4*>(srow + c0 + 4);
+    ra[0] = __float_as_uint(x0.x); ra[1] = __float_as_uint(x0.y);
+    ra[2] = __float_as_uint(x0.z); ra[3] = __float_as_uint(x0.w);
+    ra[4] = __float_as_uint(x1.x); ra[5] = __float_as_uint(x1.y);
+    ra[6] = __float_as_uint(x1.z); ra[7] = __float_as_uint(x1.w);
+    emit(ra, c0);
   }
 }
 
@@ -499,24 +672,10 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   }
   pdl_wait();      // everything above overlapped the previous kernel's tail; global reads start here
   if (HALO && threadIdx.x == 0) {
-    // the (8 + KY - 1) x (8 + KX - 1) window of each of the tile's two 8x8 blocks, one 8-channel
-    // plane per TMA box; out-of-image positions (padding, ragged edges, a block past the last
-    // image) arrive as zeros
-    const ConvGeomU& g = p.g;
-    const int nplanes = (GKIND == G_IM2COL ? g.C : g.F) / 8, plane = halo_plane_bytes(g);
-    mbar_arrive_expect_tx(&halo_bar, 2u * nplanes * (8 + g.KY - 1) * (8 + g.KX - 1) * 16);
+    // the windows of the tile's two 8x8 blocks
+    mbar_arrive_expect_tx(&halo_bar, 2u * halo_tx_bytes<GKIND>(p));
 #pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
-      const int b = blockIdx.y * 2 + h;
-      const int bx = b % p.hnbx, b2 = b / p.hnbx, by = b2 % p.hnby, n = b2 / p.hnby;
-      // fprop: output pixel (y, x) with tap (ky, kx) reads x[y + ky - PT][x + kx - PL];
-      // dgrad: input pixel (y, x) reads err_out[y + PT - ky][x + PL - kx]
-      const int x0 = GKIND == G_IM2COL ? bx * 8 - g.PL : bx * 8 + g.PL - (g.KX - 1);
-      const int y0 = GKIND == G_IM2COL ? by * 8 - g.PT : by * 8 + g.PT - (g.KY - 1);
-#pragma unroll 1
-      for (int c = 0; c < nplanes; ++c)
-        tma_load_4d(halo + h * p.hbytes + c * plane, &tmap_a, &halo_bar, c * 8, x0, y0, n);
-    }
+    for (int h = 0; h < 2; ++h) load_halo<GKIND>(halo + h * p.hbytes, &tmap_a, &halo_bar, p, blockIdx.y * 2 + h);
   }
   if (threadIdx.x < BLOCK_N) {
     const int n = blockIdx.x * BLOCK_N + threadIdx.x;
@@ -760,9 +919,7 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 
   // ===================== epilogue =====================
   // The accumulator fragments go through shared memory (the ring is idle: every k-block has been
-  // consumed) so that thread t owns row m0 + t; the epilogue proper is then a rolled loop over
-  // 8-column chunks (it runs once per tile, so every instruction of it is an instruction-cache
-  // miss: a short loop body fetched once beats an unrolled one), output mode decided once.
+  // consumed) so that thread t owns row m0 + t.
   float* const stg = reinterpret_cast<float*>(tiles);
   {
     const int r0 = 16 * warp + (lane >> 2), cq = 2 * (lane & 3);
@@ -778,133 +935,137 @@ gemm_umma_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
   }
   named_bar_sync(1, 128);
-  enum { EPI_BF16, EPI_RAW_T, EPI_RAW, EPI_SLOW, EPI_NONE, EPI_BIASROW, EPI_F32 };
-  {
-    const int row = HALO ? halo_row<GKIND>(p, threadIdx.x) : m0 + (int)threadIdx.x;
-    const bool raw32 = !p.out_bf16 && p.beta == 0.f && p.alpha == 1.f && !p.bias && p.act == 0;
-    float* const rbase = reinterpret_cast<float*>(p.out) +
-                         (p.split_stride > 0 ? (long long)blockIdx.z * p.split_stride : 0LL);
-    int mode;
-    if (row < 0) mode = EPI_NONE;
-    else if (row >= p.M) mode = (p.bias_out && row == p.M) ? EPI_BIASROW : EPI_NONE;
-    else if (p.split_stride == 0 && !p.out_trans && p.out_bf16 && p.beta == 0.f) mode = EPI_BF16;
-    else if (p.split_stride == 0 && !p.out_trans && !p.out_bf16 && p.beta == 0.f && !raw32)
-      mode = EPI_F32;        // fp32 row-major with bias / activation (LSTM gate pre-activations,
-                             // softmax logits): same inline path as bf16, fp32 stores
-    else if (raw32 && p.out_trans) mode = EPI_RAW_T;
-    else if (raw32 && (p.ldo & 3) == 0 && (reinterpret_cast<uintptr_t>(rbase) & 15) == 0)
-      mode = EPI_RAW;
-    else mode = EPI_SLOW;
-    const float* const srow = stg + threadIdx.x * SROW;
+  const int row = HALO ? halo_row<GKIND>(p, blockIdx.y * 2 + (threadIdx.x >> 6), threadIdx.x & 63)
+                       : m0 + (int)threadIdx.x;
+  epilogue_row(p, row, stg + threadIdx.x * SROW, s_bias, n0, 0, BLOCK_N, blockIdx.z);
+}
 
-    auto emit = [&](const uint32_t (&r)[8], int c0) {
-      const int nb = n0 + c0;
-      if (mode == EPI_NONE) return;
-      if (mode == EPI_BIASROW) {       // product row M = column sums of err (see ConvGeomU::ones)
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (nb + j < p.N) p.bias_out[(long long)blockIdx.z * p.N + nb + j] = __uint_as_float(r[j]);
-        return;
-      }
-      if (mode == EPI_BF16 || mode == EPI_F32) {
-        float v[8];
-        {
-          const float4 b0 = *reinterpret_cast<const float4*>(s_bias + c0);
-          const float4 b1 = *reinterpret_cast<const float4*>(s_bias + c0 + 4);
-          v[0] = b0.x; v[1] = b0.y; v[2] = b0.z; v[3] = b0.w;
-          v[4] = b1.x; v[5] = b1.y; v[6] = b1.z; v[7] = b1.w;
-        }
-        // activation selected once per chunk (not per element): the executed path stays short
-        switch (p.act) {
-          // out = act(alpha * acc + bias): alpha is the err_input_alpha of dgrad (no bias,
-          // linear); every other caller passes alpha = 1
-          case ACT_LINEAR:
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = fmaf(__uint_as_float(r[j]), p.alpha, v[j]);
-            break;
-          case ACT_STRICT_RELU:
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = fmaxf(fmaf(__uint_as_float(r[j]), p.alpha, v[j]), 0.f);
-            break;
-          case ACT_TANH:
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              v[j] = 1.7159f * tanh_approx(0.6666f * fmaf(__uint_as_float(r[j]), p.alpha, v[j]));
-            break;
-          default:
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              v[j] = act_fwd5_fast(p.act, fmaf(__uint_as_float(r[j]), p.alpha, v[j]));
-        }
-        if (p.dmul != nullptr && mode == EPI_BF16) {
-          // err_input *= f'(x): x has the layout of the output (row pitch ldo)
-          const __nv_bfloat16* dx = p.dmul + (long long)row * p.ldo + nb;
-          if (nb + 8 <= p.N && (p.ldo & 7) == 0) {
-            float xv[8];
-            ld8(dx, xv);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] *= act_deriv(p.dact, 0.f, xv[j]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (nb + j < p.N) v[j] *= act_deriv(p.dact, 0.f, __bfloat162float(dx[j]));
-          }
-        }
-        if (mode == EPI_F32) {
-          float* qf = reinterpret_cast<float*>(p.out) + (long long)row * p.ldo + nb;
-          if (nb + 8 <= p.N && (p.ldo & 3) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
-            reinterpret_cast<float4*>(qf)[0] = make_float4(v[0], v[1], v[2], v[3]);
-            reinterpret_cast<float4*>(qf)[1] = make_float4(v[4], v[5], v[6], v[7]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (nb + j < p.N) qf[j] = v[j];
-          }
-          return;
-        }
-        __nv_bfloat16* q = reinterpret_cast<__nv_bfloat16*>(p.out) + (long long)row * p.ldo + nb;
-        if (nb + 8 <= p.N && (p.ldo & 7) == 0) {
-          st8(q, v);                   // bf16 pack: one 16-byte store per 8 outputs
-        } else {                       // ragged last chunk / row pitch not a multiple of 16 bytes
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (nb + j < p.N) q[j] = __float2bfloat16_rn(v[j]);
-        }
-      } else if (mode == EPI_RAW_T) {
-        // raw fp32 (split-K partials / FC weight gradients), transposed: for a fixed column the
-        // 32 lanes hold consecutive rows = one coalesced 128-byte store per column
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (nb + j < p.N) rbase[(long long)(nb + j) * p.ldo + row] = __uint_as_float(r[j]);
-      } else if (mode == EPI_RAW && nb + 8 <= p.N) {
-        float4* q = reinterpret_cast<float4*>(rbase + (long long)row * p.ldo + nb);
-        q[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]),
-                           __uint_as_float(r[3]));
-        q[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]),
-                           __uint_as_float(r[7]));
-      } else if (raw32) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (nb + j < p.N) rbase[(long long)row * p.ldo + nb + j] = __uint_as_float(r[j]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j)     // (static indices: r stays in registers)
-          if (nb + j < p.N) epi_store_slow(p, row, nb + j, __uint_as_float(r[j]), blockIdx.z);
-      }
-    };
+// ---- persistent halo conv: the A_HALO geometries with N <= 64 (dgrad: 16 < C <= 64) and a filter
+// that fits shared memory. A work item is one 8x8 block of output (dgrad: input) pixels x BLOCK_N
+// columns: one m64 x BLOCK_N
+// accumulator chain over every k16 step of the reduction, with the same per-step halo offsets
+// (build_halo_tab) in the same order as A_HALO, so the results are bit-identical to it. Each CTA
+// loads its BLOCK_N columns of B into shared memory once and keeps them for all its items, instead
+// of streaming the whole filter through a ring per 128-row tile. Items are taken in a static stride,
+// item = blockIdx.x + j * gridDim.x; the column tile is item % ntiles, the same for every item of a
+// CTA because gridDim.x is a multiple of ntiles. Thread 0 keeps PH_STAGES halos in flight: the halo
+// of item j + PH_STAGES is requested as soon as the MMAs of item j have retired, so its TMA overlaps
+// the epilogue and the following items. One warpgroup per CTA; the several CTAs that fit an SM
+// overlap one CTA's epilogue with another's MMAs. Resident B, one tile of BLOCK_N * 128 bytes per
+// k-block of 64 reduction indices:
+//   fprop, B = w_lp [F][ldw] (K-major): SW128 tiles [BLOCK_N rows][64], as in gemm_umma_k's ring;
+//   dgrad, B = wd_lp [Kd][ldc] (MN-major, BLOCK_N = 32): SW64 tiles [64 k-rows][32 columns], one
+//   TMA box {32, 64} each. A 64-byte row holds the 32 columns of one k-row, 8 k-rows make one
+//   512-byte swizzle atom (SBO), and a k16 step is two atoms. The SW128 MN-major tiles of
+//   gemm_umma_k are 64 columns wide, so C = 32 would issue N = 64; this issues N = 32.
+constexpr int PH_STAGES = 4;
+constexpr int PERSIST_SMEM_MAX = 226 * 1024;     // + the static barriers <= 227 KB per block
 
+__host__ __device__ __forceinline__ int persist_b_bytes(const GemmParams& p, int bn) {
+  return (p.K + BLOCK_K - 1) / BLOCK_K * bn * 128;
+}
+// dynamic shared memory of conv_halo_persist_k: alignment slack, resident B, the halo ring, the
+// fp32 staging of one item, the per-k16-step halo offsets, the bias slice
+__host__ __device__ __forceinline__ int persist_smem_bytes(const GemmParams& p, int bn) {
+  return 1024 + persist_b_bytes(p, bn) + PH_STAGES * p.hbytes + 64 * (bn + 4) * 4 +
+         ((p.ktab_n + 3) & ~3) * 4 + bn * 4;
+}
+
+template <int BLOCK_N, int GKIND>
+__global__ void __launch_bounds__(128)
+conv_halo_persist_k(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                    const GemmParams p) {
+  pdl_trigger();
+  constexpr int ACC = BLOCK_N / 2;
+  constexpr int SROW = BLOCK_N + 4;
+  constexpr bool DGRAD = GKIND == G_DGRAD;
+  static_assert(!DGRAD || BLOCK_N == 32, "dgrad B tiles are one 64-byte swizzle atom wide");
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t b_bar;
+  __shared__ __align__(8) uint64_t full_bar[PH_STAGES];
+
+  uint8_t* const bres = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  const int kb = (p.K + BLOCK_K - 1) / BLOCK_K;
+  uint8_t* const halo = bres + persist_b_bytes(p, BLOCK_N);
+  float* const stg = reinterpret_cast<float*>(halo + PH_STAGES * p.hbytes);
+  int* const tab = reinterpret_cast<int*>(stg + 64 * SROW);
+  float* const s_bias = reinterpret_cast<float*>(tab + ((p.ktab_n + 3) & ~3));
+
+  const int ntiles = (p.N + BLOCK_N - 1) / BLOCK_N;
+  const int n0 = (int)(blockIdx.x % ntiles) * BLOCK_N;
+  const int items = p.g.N * p.hnby * p.hnbx * ntiles;
+  const int nj = (items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const uint32_t hx = halo_tx_bytes<GKIND>(p);
+
+  if (threadIdx.x == 0) {
+    mbar_init(&b_bar, 1u);
+    for (int s = 0; s < PH_STAGES; ++s) mbar_init(&full_bar[s], 1u);
+    fence_barrier_init();
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+  }
+  build_halo_tab<GKIND>(tab, p);
+  pdl_wait();      // everything above overlapped the previous kernel's tail; global reads start here
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(&b_bar, (uint32_t)persist_b_bytes(p, BLOCK_N));
 #pragma unroll 1
-    for (int c0 = 0; c0 < BLOCK_N; c0 += 8) {
-      if (n0 + c0 >= p.N) break;     // chunk beyond the last column
-      uint32_t ra[8];
-      const float4 x0 = *reinterpret_cast<const float4*>(srow + c0);
-      const float4 x1 = *reinterpret_cast<const float4*>(srow + c0 + 4);
-      ra[0] = __float_as_uint(x0.x); ra[1] = __float_as_uint(x0.y);
-      ra[2] = __float_as_uint(x0.z); ra[3] = __float_as_uint(x0.w);
-      ra[4] = __float_as_uint(x1.x); ra[5] = __float_as_uint(x1.y);
-      ra[6] = __float_as_uint(x1.z); ra[7] = __float_as_uint(x1.w);
-      emit(ra, c0);
+    for (int i = 0; i < kb; ++i) {
+      if (DGRAD) tma_load_2d(bres + i * (BLOCK_N * 128), &tmap_b, &b_bar, n0, i * BLOCK_K);
+      else tma_load_2d(bres + i * (BLOCK_N * 128), &tmap_b, &b_bar, i * BLOCK_K, n0);
     }
+#pragma unroll 1
+    for (int j = 0; j < PH_STAGES && j < nj; ++j) {
+      mbar_arrive_expect_tx(&full_bar[j], hx);
+      load_halo<GKIND>(halo + j * p.hbytes, &tmap_a, &full_bar[j], p,
+                       ((int)blockIdx.x + j * (int)gridDim.x) / ntiles);
+    }
+  }
+  if (threadIdx.x < BLOCK_N) {
+    const int n = n0 + threadIdx.x;
+    s_bias[threadIdx.x] = (p.bias && n < p.N) ? __ldg(p.bias + n) : 0.f;
+  }
+  __syncthreads();
+  mbar_wait(&b_bar, 0);
+
+  const uint32_t bres_sa = smem_u32(bres), halo_sa = smem_u32(halo);
+  const uint32_t halo_sbo = (8 + p.g.KX - 1) * 16;       // one halo row = the next 8 block rows
+  const int r = threadIdx.x & 63, half = threadIdx.x >> 6;  // epilogue: row and column half
+#pragma unroll 1
+  for (int j = 0; j < nj; ++j) {
+    const int s = j % PH_STAGES, item = (int)blockIdx.x + j * (int)gridDim.x;
+    const uint32_t hs = halo_sa + s * p.hbytes;
+    float acc[ACC];
+#pragma unroll
+    for (int e = 0; e < ACC; ++e) acc[e] = 0.f;
+    mbar_wait(&full_bar[s], (j / PH_STAGES) & 1);
+    wg_fence_regs(acc);
+    wg_fence();
+#pragma unroll 1
+    for (int i = 0; i < kb; ++i) {
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / 16; ++k) {
+        const int step = i * (BLOCK_K / 16) + k;
+        const uint32_t e = (uint32_t)tab[step];
+        const uint64_t da = make_smem_desc_interleave(hs + (e & 0xFFFFu), e >> 16, halo_sbo);
+        const uint64_t db = DGRAD ? make_smem_desc(bres_sa + i * (BLOCK_N * 128) + k * 1024, 0, 512, SW64)
+                                  : make_smem_desc(bres_sa + i * (BLOCK_N * 128) + k * 32, 16, 1024);
+        wgmma_bf16<BLOCK_N, 0, DGRAD ? 1 : 0>(acc, da, db, 1);
+      }
+    }
+    wg_commit();
+    wg_fence_regs(acc);
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    if (threadIdx.x == 0 && j + PH_STAGES < nj) {   // slot s is free: the halo of item j + PH_STAGES
+      mbar_arrive_expect_tx(&full_bar[s], hx);
+      load_halo<GKIND>(halo + s * p.hbytes, &tmap_a, &full_bar[s], p, (item + PH_STAGES * (int)gridDim.x) / ntiles);
+    }
+    if (j > 0) named_bar_sync(1, 128);               // the previous item's staging has been read
+    stage_acc<BLOCK_N>(stg, 0, acc);
+    named_bar_sync(1, 128);
+    epilogue_row<false>(p, halo_row<GKIND>(p, item / ntiles, r), stg + r * SROW, s_bias, n0,
+                        half * (BLOCK_N / 2), (half + 1) * (BLOCK_N / 2), 0);
   }
 }
 
@@ -926,17 +1087,19 @@ static EncodeTiledFn get_encode() {
 }
 
 // 2-D bf16 tensor map: inner dim `inner` (contiguous), outer dim `outer`, row pitch ld elements,
-// box {64, box_rows}, SWIZZLE_128B, OOB -> zeros.
+// box {64, box_rows} with SWIZZLE_128B, or {32, box_rows} with SWIZZLE_64B (box_inner = 32: the
+// dgrad B tiles of conv_halo_persist_k), OOB -> zeros.
 static int make_map(CUtensorMap* m, const void* ptr, long long inner, long long outer, long long ld,
-                    int box_rows) {
+                    int box_rows, int box_inner = 64) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return -1;
   cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
   cuuint64_t strides[1] = {(cuuint64_t)(ld * 2)};
-  cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+  cuuint32_t box[2] = {(cuuint32_t)box_inner, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1u, 1u};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box,
-                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   box_inner == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
@@ -1032,6 +1195,48 @@ static bool band_eligible(GemmParams& p) {
   p.hbytes = np * p.bplane + 128;
   return p.hbytes <= BAND_MAX_BYTES;
 }
+// ZNICZ_CONV_HALO_PERSIST=0 runs the shapes that conv_halo_persist_k serves on A_HALO instead
+static bool halo_persist_enabled() {
+  static int on = -1;
+  if (on < 0) { const char* e = getenv("ZNICZ_CONV_HALO_PERSIST"); on = (e && atoi(e) == 0) ? 0 : 1; }
+  return on != 0;
+}
+// The persistent kernel's column tile for an A_HALO shape (p from halo_eligible) with N columns,
+// and the shared memory it needs; 0 when it does not serve the shape: N > 64, an output other than
+// bf16 without beta (see epilogue_row<false>), or a resident B and halo ring that do not fit.
+// p.ktab_n is set to the k16 steps (build_halo_tab).
+static int persist_bn(GemmParams& p, int& smem) {
+  if (!halo_persist_enabled() || p.N > 64 || !p.out_bf16 || p.beta != 0.f) return 0;
+  const int bn = p.N <= 16 ? 16 : 32;      // N = 64: two 32-column items per block, more items
+  p.ktab_n = (p.K + BLOCK_K - 1) / BLOCK_K * (BLOCK_K / 16);
+  smem = persist_smem_bytes(p, bn);
+  return smem <= PERSIST_SMEM_MAX ? bn : 0;
+}
+// Grid: as many CTAs as fit at once (occupancy at this shared-memory size), reduced to the fewest
+// that still give every CTA the same number of items +- 1 in as many rounds (fewer CTAs load B
+// fewer times), rounded up to a multiple of the column tiles.
+template <int BN, int GK>
+static int launch_persist(const CUtensorMap& th, const CUtensorMap& tb, const GemmParams& p, int smem,
+                          cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(conv_halo_persist_k<BN, GK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         PERSIST_SMEM_MAX);
+    if (e != cudaSuccess) return (int)e;
+    attr_set = true;
+  }
+  int occ = 0;
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, conv_halo_persist_k<BN, GK>, 128, smem);
+  if (e != cudaSuccess) return (int)e;
+  if (occ < 1) return -6;
+  const long long ntiles = (p.N + BN - 1) / BN, items = (long long)p.g.N * p.hnby * p.hnbx * ntiles;
+  const long long slots = (long long)occ * num_sms(), rounds = (items + slots - 1) / slots;
+  long long grid = (items + rounds - 1) / rounds;
+  grid = std::min(items, (grid + ntiles - 1) / ntiles * ntiles);
+  launch_k(conv_halo_persist_k<BN, GK>, dim3((unsigned)grid), 128, smem, st, th, tb, p);
+  return (int)cudaGetLastError();
+}
+
 static int make_map_halo(CUtensorMap* m, const void* ptr, int N, int H, int W, int C, int KY, int KX,
                          int box_w = 0, int box_h = 0) {
   EncodeTiledFn enc = get_encode();
@@ -1250,6 +1455,14 @@ int launch_conv_fprop_umma(const void* x, const void* w_lp, long long ldw, const
       r = make_map_halo(&th, x, N, H, W, C, KY, KX);
       if (r) return r;
       ++g_halo_launches;
+      int smem = 0;
+      if (const int pbn = persist_bn(p, smem)) {
+        CUtensorMap tp;                          // B box {64, pbn}
+        r = make_map(&tp, w_lp, ldw, F, ldw, pbn);
+        if (r) return r;
+        return pbn == 16 ? launch_persist<16, G_IM2COL>(th, tp, p, smem, st)
+                         : launch_persist<32, G_IM2COL>(th, tp, p, smem, st);
+      }
       return launch_bn<A_HALO, B_TMA_K, G_IM2COL, 0>(bn, th, tb, p, 1, st);
     }
     return launch_bn<A_GATHER_K, B_TMA_K, G_IM2COL, 2>(bn, ta, tb, p, 1, st);
@@ -1308,6 +1521,13 @@ int launch_conv_dgrad_umma(const void* err_out, const void* wd_lp, long long ldc
       r = make_map_halo(&th, err_out, N, OH, OW, F, KY, KX);
       if (r) return r;
       ++g_halo_launches;
+      int smem = 0;
+      if (persist_bn(p, smem) == 32) {          // C <= 16 keeps A_HALO (B tiles are 32 columns)
+        CUtensorMap tp;                          // B box {32, 64}, SWIZZLE_64B
+        r = make_map(&tp, wd_lp, ldc, Kd, ldc, BLOCK_K, 32);
+        if (r) return r;
+        return launch_persist<32, G_DGRAD>(th, tp, p, smem, st);
+      }
       return launch_bn<A_HALO, B_TMA_MN, G_DGRAD, 0>(bn, th, tb, p, 1, st);
     }
     return launch_bn<A_GATHER_K, B_TMA_MN, G_DGRAD, 2>(bn, ta, tb, p, 1, st);

@@ -247,13 +247,15 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 //   [32,46) stride-dim byte offset >> 4     [49,52) base offset = 0     [62,64) layout = 1 (SW128)
 // K-major: 128-byte rows, 8-row groups SBO = 1024 apart (LBO unused). MN-major: 64-element rows
 // along M / N, 8 k-rows per 1024-byte atom (SBO = 1024), next 64 M / N columns LBO bytes further.
+// layout = SW64 (2): the same with 64-byte rows (32 elements), 8-row atoms of 512 bytes.
+enum : uint32_t { SW128 = 1, SW64 = 2 };
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes) {
+                                                   uint32_t sbo_bytes, uint32_t layout = SW128) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 62;
+  d |= (uint64_t)layout << 62;
   return d;
 }
 // The same descriptor without swizzle (layout = 0, "interleave"), K-major: a core matrix is 8 rows
