@@ -408,9 +408,23 @@ def _update(unit, is_bias, grad_buf, nparts, part_stride, rows, cols, g_cpad=0):
     else:
         ptrs, flag_ptrs, epoch_ptr, blocks, rank = [grad_buf.data_ptr()], [], 0, 0, 0
     wdev = w.dev
-    gout_dev = gout.dev_out if gout else None
+    if flags & unit.FLAG_RPROP:
+        if not gout:
+            raise RuntimeError("%s: RProp keeps the previous gradient in gradient_%s" %
+                               (unit, "bias" if is_bias else "weights"))
+        gout_dev = gout.dev          # read (previous gradient) and rewritten by the kernel
+        gout.dev_written()
+    else:
+        gout_dev = gout.dev_out if gout else None
     acc_dev = acc.dev if acc else None
     vel_dev = vel.dev if vel else None
+    # solver state (adagrad / adadelta / fast / RProp): stepped in the same kernel
+    states = [a if a is not None and a else None for a in unit.solver_arrays(for_bias=is_bias)]
+    for bit, a in ((unit.FLAG_ADAGRAD | unit.FLAG_ADADELTA | unit.FLAG_RPROP, states[0]),
+                   (unit.FLAG_ADADELTA, states[1]), (unit.FLAG_FAST, states[2])):
+        if (flags & bit) and a is None:
+            raise RuntimeError("%s: solver state missing for flags %#x" % (unit, flags))
+    sdev = [a.dev if a is not None else None for a in states]
     if step is not None:
         # deferred: the whole-network step kernel applies it (ops/fused_step.py)
         size = wdev.numel()
@@ -424,14 +438,16 @@ def _update(unit, is_bias, grad_buf, nparts, part_stride, rows, cols, g_cpad=0):
                    p(colsums)] + [int(x) for x in ptrs] + [0] * (8 - len(ptrs)) +
                   [int(part_stride), int(size), int(nparts), int(g_cpad), int(flags),
                    1 if is_bias else 0, int(rows), int(cols), lanes, 1,
-                   p(lp), int(ld), int(cpad_lp), p(lp_conv), int(taps), int(c), int(c_pad)])
+                   p(lp), int(ld), int(cpad_lp), p(lp_conv), int(taps), int(c), int(c_pad)] +
+                  [p(t) for t in sdev])
         step.submit(unit, is_bias, fields,
-                    (wdev, gout_dev, acc_dev, vel_dev, colsums, lp, lp_conv, grad_buf),
+                    (wdev, gout_dev, acc_dev, vel_dev, colsums, lp, lp_conv, *sdev, grad_buf),
                     grad_buf.data_ptr())
     else:
         ext.fused_update(wdev, ptrs, nparts, part_stride, gout_dev, acc_dev, vel_dev,
                          unit.hyper_dev_, colsums, flags, is_bias, rows, cols, lp, ld, lp_conv,
-                         taps, c, c_pad, flag_ptrs, epoch_ptr, rank, blocks, cpad_lp, g_cpad)
+                         taps, c, c_pad, flag_ptrs, epoch_ptr, rank, blocks, cpad_lp, g_cpad,
+                         *sdev)
         _launch()
         if not is_bias and getattr(fwd, "weights_q_", None) is not None:
             requantize_weights(fwd)
@@ -440,6 +456,9 @@ def _update(unit, is_bias, grad_buf, nparts, part_stride, rows, cols, g_cpad=0):
         acc.dev_written()
     if vel:
         vel.dev_written()
+    for a in states:
+        if a is not None:
+            a.dev_written()
     if dp is not None and dp.symm is None and dp.world_size > 1 and step is None:
         raise RuntimeError("the NCCL baseline mode needs the fused step (engine.fused_step)")
 

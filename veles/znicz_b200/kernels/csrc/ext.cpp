@@ -40,7 +40,7 @@ void launch_evaluate_softmax(const float*, const int*, const int*, void*, bool, 
 void launch_evaluate_mse(const void*, const void*, bool, void*, bool, const float*, int, int, const float*, int, float*, float*, cudaStream_t);
 void launch_mse_find_closest(const void*, bool, const float*, const int*, const float*, int, int, int, int*, cudaStream_t);
 int fused_update_blocks(long long size);
-void launch_fused_update(float*, const float* const*, int, int, long long, float*, float*, float*, const float*, const float*, int, int, long long, int, int, __nv_bfloat16*, int, __nv_bfloat16*, int, int, int, uint32_t* const*, uint32_t*, int, int, int, int, cudaStream_t);
+void launch_fused_update(float*, const float* const*, int, int, long long, float*, float*, float*, const float*, const float*, int, int, long long, int, int, __nv_bfloat16*, int, __nv_bfloat16*, int, int, int, uint32_t* const*, uint32_t*, int, int, int, int, float*, float*, float*, cudaStream_t);
 void launch_col_sums(const float*, float*, int, int, int, cudaStream_t);
 void launch_lstm_cell_fwd(const float*, const float*, float*, float*, void*, long long, void*, long long, int, int, bool, cudaStream_t);
 void launch_lstm_cell_bwd(const void*, long long, const void*, long long, const float*, const float*, const float*, const float*, float*, void*, int, int, bool, cudaStream_t);
@@ -510,8 +510,22 @@ void fused_update(Tensor w, std::vector<int64_t> grad_ptrs, int64_t nparts, int6
                   Tensor hyper, c10::optional<Tensor> col_sums, int64_t flags, bool is_bias, int64_t rows,
                   int64_t cols, c10::optional<Tensor> lp, int64_t ld, c10::optional<Tensor> lp_conv,
                   int64_t taps, int64_t C, int64_t c_pad, std::vector<int64_t> peer_flags,
-                  int64_t epoch_ptr, int64_t rank, int64_t blocks, int64_t lp_cpad, int64_t g_cpad) {
+                  int64_t epoch_ptr, int64_t rank, int64_t blocks, int64_t lp_cpad, int64_t g_cpad,
+                  c10::optional<Tensor> s0, c10::optional<Tensor> s1, c10::optional<Tensor> s2) {
   TORCH_CHECK(w.scalar_type() == torch::kFloat32 && w.is_cuda() && w.is_contiguous());
+  // solver state (update.cu::step_elem): s0 adagrad h / adadelta E[dx^2] / RProp lrs,
+  // s1 adadelta E[g^2], s2 fast f; each one element per weight
+  for (const auto* t : {&s0, &s1, &s2})
+    TORCH_CHECK(!t->has_value() || !(*t)->defined() || (*t)->numel() == 0 || (*t)->numel() == w.numel(),
+                "fused_update: solver state must match the weights");
+  TORCH_CHECK(!(flags & 256) || (mfptr_or_null(grad_out) && mfptr_or_null(s0)),
+              "fused_update: RProp needs grad_out (previous gradient) and the rates");
+  TORCH_CHECK(!(flags & (32 | 64)) || mfptr_or_null(s0), "fused_update: adagrad / adadelta need s0");
+  TORCH_CHECK(!(flags & 64) || mfptr_or_null(s1), "fused_update: adadelta needs s1");
+  TORCH_CHECK(!(flags & 128) || mfptr_or_null(s2), "fused_update: fast needs s2");
+  TORCH_CHECK(hyper.is_cuda() && hyper.scalar_type() == torch::kFloat32 &&
+              hyper.numel() >= ((flags & (32 | 64 | 128 | 256)) ? 21 : 13),
+              "fused_update: the hyper vector is too short (solver slots 13-20)");
   TORCH_CHECK(grad_ptrs.size() >= 1 && grad_ptrs.size() <= 8);
   const float* gp[8]; uint32_t* fl[8];
   for (size_t i = 0; i < grad_ptrs.size(); ++i) gp[i] = reinterpret_cast<const float*>(grad_ptrs[i]);
@@ -523,14 +537,26 @@ void fused_update(Tensor w, std::vector<int64_t> grad_ptrs, int64_t nparts, int6
                           w.numel(), (int)rows, (int)cols, bptr_or_null(lp), (int)ld, bptr_or_null(lp_conv),
                           (int)taps, (int)C, (int)c_pad, multi ? fl : nullptr,
                           reinterpret_cast<uint32_t*>(epoch_ptr), (int)rank, (int)blocks, (int)lp_cpad,
-                          (int)g_cpad, cur());
+                          (int)g_cpad, mfptr_or_null(s0), mfptr_or_null(s1), mfptr_or_null(s2), cur());
   kcheck();
+}
+// the form without solver state (plain SGD / momentum / accumulation)
+void fused_update_sgd(Tensor w, std::vector<int64_t> grad_ptrs, int64_t nparts, int64_t part_stride,
+                      c10::optional<Tensor> grad_out, c10::optional<Tensor> acc, c10::optional<Tensor> vel,
+                      Tensor hyper, c10::optional<Tensor> col_sums, int64_t flags, bool is_bias, int64_t rows,
+                      int64_t cols, c10::optional<Tensor> lp, int64_t ld, c10::optional<Tensor> lp_conv,
+                      int64_t taps, int64_t C, int64_t c_pad, std::vector<int64_t> peer_flags,
+                      int64_t epoch_ptr, int64_t rank, int64_t blocks, int64_t lp_cpad, int64_t g_cpad) {
+  fused_update(w, grad_ptrs, nparts, part_stride, grad_out, acc, vel, hyper, col_sums, flags, is_bias, rows,
+               cols, lp, ld, lp_conv, taps, C, c_pad, peer_flags, epoch_ptr, rank, blocks, lp_cpad, g_cpad,
+               c10::nullopt, c10::nullopt, c10::nullopt);
 }
 int64_t update_blocks(int64_t size) { return zn::fused_update_blocks(size); }
 
-// Whole-network step table. Each descriptor is 31 int64 fields:
+// Whole-network step table. Each descriptor is 31 to 34 int64 fields:
 // [w, grad_out, acc, vel, hyper, col_sums, grad[0..7], part_stride, size, nparts, g_cpad, flags,
-//  is_bias, rows, cols, lanes, enabled, lp, ld, lp_cpad, lp_conv, taps, C, c_pad]
+//  is_bias, rows, cols, lanes, enabled, lp, ld, lp_cpad, lp_conv, taps, C, c_pad
+//  (, s0, s1, s2: solver state, null when absent)]
 // Returns (packed CPU uint8 tensor [n * desc_size], total_tiles).
 std::tuple<Tensor, int64_t, int64_t> multi_update_table(std::vector<std::vector<int64_t>> descs, int64_t red_base) {
   const size_t ds = zn::multi_update_desc_size();
@@ -540,9 +566,16 @@ std::tuple<Tensor, int64_t, int64_t> multi_update_table(std::vector<std::vector<
   int tiles = 0;
   long long red = red_base;
   for (size_t i = 0; i < descs.size(); ++i) {
-    TORCH_CHECK(descs[i].size() == 31, "descriptor must have 31 fields");
+    const int nf = (int)descs[i].size();
+    TORCH_CHECK(nf >= 31 && nf <= 34, "descriptor must have 31 to 34 fields");
     std::vector<long long> f(descs[i].begin(), descs[i].end());
-    tiles += zn::multi_update_pack(f.data(), 31, out.data_ptr<uint8_t>() + i * ds, tiles, red);
+    const long long fl = f[18];
+    auto has = [&](int k) { return nf > k && f[k] != 0; };
+    TORCH_CHECK(!(fl & 256) || (f[1] != 0 && has(31)), "RProp needs grad_out and the rates (field 31)");
+    TORCH_CHECK(!(fl & (32 | 64)) || has(31), "adagrad / adadelta need state field 31");
+    TORCH_CHECK(!(fl & 64) || has(32), "adadelta needs state field 32");
+    TORCH_CHECK(!(fl & 128) || has(33), "fast needs state field 33");
+    tiles += zn::multi_update_pack(f.data(), nf, out.data_ptr<uint8_t>() + i * ds, tiles, red);
     // one fp32 slot per element in the cross-GPU reduction buffer; every tensor starts on a
     // 16-byte boundary (the 4-elements-per-thread tile path uses float4 accesses)
     red += (f[15] + 3) / 4 * 4;
@@ -1080,7 +1113,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("lrn_forward", &lrn_forward); m.def("lrn_backward", &lrn_backward);
   m.def("softmax_rows", &softmax_rows); m.def("evaluate_softmax", &evaluate_softmax);
   m.def("evaluate_mse", &evaluate_mse); m.def("mse_find_closest", &mse_find_closest);
-  m.def("fused_update", &fused_update); m.def("update_blocks", &update_blocks);
+  m.def("fused_update", &fused_update_sgd); m.def("fused_update", &fused_update);
+  m.def("update_blocks", &update_blocks);
   m.def("som_split", &som_split); m.def("split_parts", &split_parts); m.def("split_conv_wt", &split_conv_wt); m.def("som_argmin", &som_argmin);
   m.def("som_gravity_split", &som_gravity_split); m.def("som_apply", &som_apply);
   m.def("multi_update_table", &multi_update_table);

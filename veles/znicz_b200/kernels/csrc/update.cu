@@ -10,6 +10,7 @@
 //   gd   = -lr * (g + wd * ((1 - l1) * w + 0.5 * l1 * sign(w)) + ortho / rows * (colsum[col] - w))
 //   acc  = acc_beta * acc + acc_alpha * gd ; gd = gd_beta * gd + gd_alpha * acc      (optional)
 //   gd  += moment * vel ; vel = gd                                                     (optional)
+//   gd  -> adagrad or adadelta, fast weights                                          (optional)
 //   w   += gd                                                                          (optional)
 //   + bf16 shadow copies of w in the layouts the wgmma GEMM/conv kernels consume.
 //
@@ -103,13 +104,100 @@ __device__ __forceinline__ void mm_st_f4(float* mc, float4 v) {
                "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
-// hyper layout: see GradientDescentBase.HYPER_FIELDS
+// ---- the per-element step, shared by the per-tensor kernel and both paths of the whole-network
+// kernel. Bits of the flags word (GradientDescentBase.update_flags):
+enum : int {
+  UF_APPLY = 1, UF_MOMENT = 2, UF_ACC = 4, UF_ORTHO = 8, UF_TRANSPOSED = 16,
+  UF_ADAGRAD = 32, UF_ADADELTA = 64, UF_FAST = 128, UF_RPROP = 256,
+  UF_SOLVERS = UF_ADAGRAD | UF_ADADELTA | UF_FAST | UF_RPROP
+};
+
+// hyper layout: see GradientDescentBase.HYPER_FIELDS. Slots >= 13 are read only when a solver bit
+// is set (a 16-float vector without solver slots stays valid for the plain step).
+struct StepHyper {
+  float lr, wd, l1, moment, acc_alpha, acc_beta, gd_alpha, gd_beta, ortho;
+  float x0, x1, x2, x3;   // adagrad eps, adadelta rho, adadelta eps, fast lr | RProp inc, dec, min, max
+};
+
+__device__ __forceinline__ StepHyper load_step_hyper(const float* hyper, int flags, int is_bias) {
+  StepHyper h;
+  h.lr = hyper[is_bias ? 9 : 0]; h.wd = hyper[is_bias ? 10 : 1];
+  h.l1 = hyper[is_bias ? 11 : 2]; h.moment = hyper[is_bias ? 12 : 3];
+  h.acc_alpha = hyper[4]; h.acc_beta = hyper[5]; h.gd_alpha = hyper[6]; h.gd_beta = hyper[7];
+  h.ortho = hyper[8];
+  h.x0 = h.x1 = h.x2 = h.x3 = 0.f;
+  if (flags & UF_SOLVERS) {
+    const int o = (flags & UF_RPROP) ? 17 : 13;
+    h.x0 = hyper[o]; h.x1 = hyper[o + 1]; h.x2 = hyper[o + 2]; h.x3 = hyper[o + 3];
+  }
+  return h;
+}
+
+// One element. The caller loads w, the accumulator (av), the velocity (vv) and the solver state
+// (s0: adagrad h, adadelta E[dx^2], RProp lrs; s1: adadelta E[g^2]; s2: fast f) into registers and
+// stores them back afterwards. cs = column sum of the pre-update weights (ortho), prev = the
+// previous step's gradient (RProp). Order: SGD (+ accumulation) -> momentum (vv keeps this value)
+// -> adagrad | adadelta -> fast, as GDCommon.numpy_update / ops.gd.solver_step.
+// SOLVERS = false compiles the solver code out (the float4 path never sees solver bits).
+template <bool SOLVERS>
+__device__ __forceinline__ void step_elem(const StepHyper& h, const int flags, const int rows,
+                                          const float g, const float cs, const float prev, float& wv,
+                                          float& av, float& vv, float& s0, float& s1, float& s2) {
+  const bool apply = flags & UF_APPLY;
+  if (SOLVERS && (flags & UF_RPROP)) {
+    // sign-based per-weight rates on the raw gradient (ops.rprop_gd.rprop_step)
+    const float d = prev * g;
+    float r = s0;
+    if (d > 0.f) r = __fmul_rn(r, h.x0);
+    if (d < 0.f) r = __fmul_rn(r, h.x1);
+    r = fminf(fmaxf(r, h.x2), h.x3);
+    s0 = r;
+    if (apply) wv = __fsub_rn(wv, (g > 0.f ? 1.f : (g < 0.f ? -1.f : 0.f)) * r);
+    return;
+  }
+  // explicit roundings: every caller (scalar / float4, single-GPU / cross-GPU) inlines this into
+  // a different context, and free contraction into FMAs could round differently in each; the
+  // replicas and the single-GPU path must stay bit-identical
+  const float sgn = wv > 0.f ? 1.f : (wv < 0.f ? -1.f : 0.f);
+  float reg = __fmul_rn(h.wd, __fmaf_rn(1.f - h.l1, wv, 0.5f * h.l1 * sgn));
+  if (flags & UF_ORTHO) reg = __fmaf_rn(h.ortho / (float)rows, cs - wv, reg);
+  float gd = __fmul_rn(-h.lr, __fadd_rn(g, reg));
+  if (flags & UF_ACC) {
+    const float a = __fmaf_rn(h.acc_alpha, gd, h.acc_beta != 0.f ? __fmul_rn(h.acc_beta, av) : 0.f);
+    av = a;
+    gd = __fmaf_rn(gd, h.gd_beta, __fmul_rn(h.gd_alpha, a));
+  }
+  if (flags & UF_MOMENT) { gd = __fmaf_rn(vv, h.moment, gd); vv = gd; }
+  if (SOLVERS) {
+    // rounded like the numpy oracle, one operation at a time
+    if (flags & UF_ADAGRAD) {
+      s0 = __fadd_rn(s0, __fmul_rn(gd, gd));
+      gd = __fdiv_rn(gd, __fsqrt_rn(__fadd_rn(s0, h.x0)));
+    }
+    if (flags & UF_ADADELTA) {
+      const float keep = 1.f - h.x1;
+      s1 = __fadd_rn(__fmul_rn(s1, h.x1), __fmul_rn(keep, __fmul_rn(gd, gd)));
+      gd = __fdiv_rn(__fmul_rn(gd, __fsqrt_rn(__fadd_rn(s0, h.x2))), __fsqrt_rn(__fadd_rn(s1, h.x2)));
+      s0 = __fadd_rn(__fmul_rn(s0, h.x1), __fmul_rn(keep, __fmul_rn(gd, gd)));
+    }
+    if (flags & UF_FAST) {
+      s2 = __fmul_rn(s2, 0.95f);
+      if (flags & UF_MOMENT) s2 = __fadd_rn(s2, __fmul_rn(h.x3, vv));
+    }
+  }
+  if (apply) {
+    wv = __fadd_rn(wv, gd);
+    if (SOLVERS && (flags & UF_FAST) && !(flags & UF_TRANSPOSED)) wv = __fsub_rn(wv, s2);
+  }
+}
+
 template <bool MULTI>
 __global__ void fused_update_k(float* __restrict__ w, GradSources gs, float* __restrict__ grad_out,
                                float* __restrict__ acc, float* __restrict__ vel,
                                const float* __restrict__ hyper, const float* __restrict__ col_sums,
                                int flags, int is_bias, long long size, int rows, int cols,
-                               ShadowSpec sh, PeerSync ps) {
+                               ShadowSpec sh, PeerSync ps, float* __restrict__ s0p,
+                               float* __restrict__ s1p, float* __restrict__ s2p) {
   pdl_entry();
   __shared__ uint32_t s_epoch;
   uint32_t epoch = 0;
@@ -119,13 +207,9 @@ __global__ void fused_update_k(float* __restrict__ w, GradSources gs, float* __r
     epoch = s_epoch;
     peer_barrier(ps, 2 * epoch - 1);   // every rank's gradient is complete and visible
   }
-  const float lr = hyper[is_bias ? 9 : 0], wd = hyper[is_bias ? 10 : 1];
-  const float l1 = hyper[is_bias ? 11 : 2], moment = hyper[is_bias ? 12 : 3];
-  const float acc_alpha = hyper[4], acc_beta = hyper[5], gd_alpha = hyper[6], gd_beta = hyper[7];
-  const float ortho = hyper[8];
-  const bool apply = flags & 1, use_moment = flags & 2, use_acc = flags & 4;
-  const bool use_ortho = (flags & 8) && col_sums != nullptr;
-  const bool transposed = flags & 16;
+  if (col_sums == nullptr) flags &= ~UF_ORTHO;
+  const StepHyper h = load_step_hyper(hyper, flags, is_bias);
+  const bool transposed = flags & UF_TRANSPOSED;
 
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long stride = (long long)gridDim.x * blockDim.x;
@@ -151,25 +235,23 @@ __global__ void fused_update_k(float* __restrict__ w, GradSources gs, float* __r
       g += (g0 + g1) + (g2 + g3);
     }
     g *= gs.gscale;
+    // weights [rows=Y][cols=H] (or stored transposed [H][Y]); col index = input index
+    const float cs = (flags & UF_ORTHO) ? col_sums[transposed ? (int)(i / rows) : (int)(i % cols)] : 0.f;
+    const float prev = (flags & UF_RPROP) ? grad_out[i] : 0.f;
     if (grad_out) grad_out[i] = g;
     float wv = w[i];
-    float sgn = wv > 0.f ? 1.f : (wv < 0.f ? -1.f : 0.f);
-    float reg = wd * ((1.f - l1) * wv + 0.5f * l1 * sgn);
-    if (use_ortho) {
-      // weights [rows=Y][cols=H] (or stored transposed [H][Y]); col index = input index
-      int col = transposed ? (int)(i / rows) : (int)(i % cols);
-      int n_rows = transposed ? cols : rows;
-      reg += ortho / (float)(transposed ? rows : rows) * (col_sums[col] - wv);
-      (void)n_rows;
-    }
-    float gd = -lr * (g + reg);
-    if (use_acc) {
-      float a = (acc_beta != 0.f ? acc_beta * acc[i] : 0.f) + acc_alpha * gd;
-      acc[i] = a;
-      gd = gd * gd_beta + gd_alpha * a;
-    }
-    if (use_moment) { gd += vel[i] * moment; vel[i] = gd; }
-    if (apply) { wv += gd; w[i] = wv; }
+    float av = (flags & UF_ACC) && h.acc_beta != 0.f ? acc[i] : 0.f;
+    float vv = (flags & UF_MOMENT) ? vel[i] : 0.f;
+    float s0 = (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) ? s0p[i] : 0.f;
+    float s1 = (flags & UF_ADADELTA) ? s1p[i] : 0.f;
+    float s2 = (flags & UF_FAST) ? s2p[i] : 0.f;
+    step_elem<true>(h, flags, rows, g, cs, prev, wv, av, vv, s0, s1, s2);
+    if (flags & UF_ACC) acc[i] = av;
+    if (flags & UF_MOMENT) vel[i] = vv;
+    if (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) s0p[i] = s0;
+    if (flags & UF_ADADELTA) s1p[i] = s1;
+    if (flags & UF_FAST) s2p[i] = s2;
+    if (flags & UF_APPLY) w[i] = wv;
     if (sh.lp) {
       int r = (int)(i / cols), c = (int)(i % cols);
       int lc = c;
@@ -246,6 +328,7 @@ struct TensorDesc {
   int ept;                    // elements per thread (lanes == 1 only): 4 for large tensors
   int vec4;                   // ept == 4 and every array / stride is 16-byte aligned: float4 path
   long long red_off;          // offset of this tensor in the cross-GPU reduction buffer
+  float* s0; float* s1; float* s2;   // solver state (step_elem), null when unused
 };
 
 struct GridSync { unsigned* count; unsigned* gen; };
@@ -393,21 +476,17 @@ __device__ __forceinline__ void multi_elem4(const TensorDesc& d, const long long
   if (MODE == 1) { *reinterpret_cast<float4*>(rb.ptr[rb.rank] + poff + d.red_off + i0) = g4; return; }
   g4.x *= rb.gscale; g4.y *= rb.gscale; g4.z *= rb.gscale; g4.w *= rb.gscale;
 
-  const int is_bias = d.is_bias;
-  const float* hyper = d.hyper;
-  const float lr = hyper[is_bias ? 9 : 0], wd = hyper[is_bias ? 10 : 1];
-  const float l1 = hyper[is_bias ? 11 : 2], moment = hyper[is_bias ? 12 : 3];
-  const float acc_alpha = hyper[4], acc_beta = hyper[5], gd_alpha = hyper[6], gd_beta = hyper[7];
-  const float ortho = hyper[8];
-  const int flags = d.flags;
-  const bool apply = flags & 1, use_moment = flags & 2, use_acc = flags & 4;
-  const bool use_ortho = (flags & 8) && d.col_sums != nullptr;
-  const bool transposed = flags & 16;
+  // (no solver bits here: multi_update_pack sends solver tensors to the scalar 4-element path)
+  const int flags = d.col_sums != nullptr ? d.flags : (d.flags & ~UF_ORTHO);
+  const StepHyper h = load_step_hyper(d.hyper, 0, d.is_bias);
+  const bool apply = flags & UF_APPLY, use_moment = flags & UF_MOMENT, use_acc = flags & UF_ACC;
+  const bool use_ortho = flags & UF_ORTHO;
+  const bool transposed = flags & UF_TRANSPOSED;
   const int rows = d.rows, cols = d.cols;
   // ---- every load first ----
   const float4 w4 = *reinterpret_cast<const float4*>(d.w + i0);
   const float4 v4 = use_moment ? *reinterpret_cast<const float4*>(d.vel + i0) : z4;
-  const float4 c4 = (use_acc && acc_beta != 0.f) ? *reinterpret_cast<const float4*>(d.acc + i0) : z4;
+  const float4 c4 = (use_acc && h.acc_beta != 0.f) ? *reinterpret_cast<const float4*>(d.acc + i0) : z4;
   float cs[4] = {0.f, 0.f, 0.f, 0.f};
   if (use_ortho) {
 #pragma unroll
@@ -422,17 +501,8 @@ __device__ __forceinline__ void multi_elem4(const TensorDesc& d, const long long
   float av[4] = {c4.x, c4.y, c4.z, c4.w};
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const float sgn = wv[j] > 0.f ? 1.f : (wv[j] < 0.f ? -1.f : 0.f);
-    float reg = wd * ((1.f - l1) * wv[j] + 0.5f * l1 * sgn);
-    if (use_ortho) reg += ortho / (float)rows * (cs[j] - wv[j]);
-    float gd = -lr * (g[j] + reg);
-    if (use_acc) {
-      const float a = (acc_beta != 0.f ? acc_beta * av[j] : 0.f) + acc_alpha * gd;
-      av[j] = a;
-      gd = gd * gd_beta + gd_alpha * a;
-    }
-    if (use_moment) { gd += vv[j] * moment; vv[j] = gd; }
-    if (apply) wv[j] += gd;
+    float unused = 0.f;
+    step_elem<false>(h, flags, rows, g[j], cs[j], 0.f, wv[j], av[j], vv[j], unused, unused, unused);
   }
   // ---- then every store ----
   if (d.grad_out) *reinterpret_cast<float4*>(d.grad_out + i0) = g4;
@@ -556,33 +626,32 @@ __device__ __forceinline__ void multi_apply(const TensorDesc& d, const long long
   if (!valid || lane != 0) return;
   if (MODE == 1) { rb.ptr[rb.rank][poff + d.red_off + i] = g; return; }
 
-  const float* hyper = d.hyper;
-  const float lr = hyper[is_bias ? 9 : 0], wd = hyper[is_bias ? 10 : 1];
-  const float l1 = hyper[is_bias ? 11 : 2], moment = hyper[is_bias ? 12 : 3];
-  const float acc_alpha = hyper[4], acc_beta = hyper[5], gd_alpha = hyper[6], gd_beta = hyper[7];
-  const float ortho = hyper[8];
-  const int flags = d.flags;
-  const bool apply = flags & 1, use_moment = flags & 2, use_acc = flags & 4;
-  const bool use_ortho = (flags & 8) && d.col_sums != nullptr;
-  const bool transposed = flags & 16;
+  const int flags = d.col_sums != nullptr ? d.flags : (d.flags & ~UF_ORTHO);
+  const StepHyper h = load_step_hyper(d.hyper, flags, is_bias);
+  const bool transposed = flags & UF_TRANSPOSED;
   const int rows = d.rows, cols = d.cols;
 
+  const float cs = (flags & UF_ORTHO) ? d.col_sums[transposed ? (int)(i / rows) : (int)(i % cols)] : 0.f;
+  const float prev = (flags & UF_RPROP) ? d.grad_out[i] : 0.f;     // read before it is overwritten
   if (d.grad_out) d.grad_out[i] = g;
   float wv = d.w[i];
-  const float sgn = wv > 0.f ? 1.f : (wv < 0.f ? -1.f : 0.f);
-  float reg = wd * ((1.f - l1) * wv + 0.5f * l1 * sgn);
-  if (use_ortho) {
-    const int col = transposed ? (int)(i / rows) : (int)(i % cols);
-    reg += ortho / (float)rows * (d.col_sums[col] - wv);
+  float av = (flags & UF_ACC) && h.acc_beta != 0.f ? d.acc[i] : 0.f;
+  float vv = (flags & UF_MOMENT) ? d.vel[i] : 0.f;
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+  if (flags & UF_SOLVERS) {
+    if (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) s0 = d.s0[i];
+    if (flags & UF_ADADELTA) s1 = d.s1[i];
+    if (flags & UF_FAST) s2 = d.s2[i];
   }
-  float gd = -lr * (g + reg);
-  if (use_acc) {
-    const float a = (acc_beta != 0.f ? acc_beta * d.acc[i] : 0.f) + acc_alpha * gd;
-    d.acc[i] = a;
-    gd = gd * gd_beta + gd_alpha * a;
+  step_elem<true>(h, flags, rows, g, cs, prev, wv, av, vv, s0, s1, s2);
+  if (flags & UF_ACC) d.acc[i] = av;
+  if (flags & UF_MOMENT) d.vel[i] = vv;
+  if (flags & UF_SOLVERS) {
+    if (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) d.s0[i] = s0;
+    if (flags & UF_ADADELTA) d.s1[i] = s1;
+    if (flags & UF_FAST) d.s2[i] = s2;
   }
-  if (use_moment) { gd += d.vel[i] * moment; d.vel[i] = gd; }
-  if (apply) { wv += gd; d.w[i] = wv; }
+  if (flags & UF_APPLY) d.w[i] = wv;
   const ShadowSpec& sh = d.sh;
   if (sh.lp) {
     const int r = (int)(i / cols), c = (int)(i % cols);
@@ -773,12 +842,19 @@ int multi_update_pack(const long long* f, int n_fields, void* out, int tile_begi
   d.sh.lp = (__nv_bfloat16*)f[24]; d.sh.ld = (int)f[25]; d.sh.lp_cpad = (int)f[26];
   d.sh.lp_conv = (__nv_bfloat16*)f[27]; d.sh.taps = (int)f[28]; d.sh.C = (int)f[29];
   d.sh.c_pad = (int)f[30];
+  // fields 31-33 (solver state) are optional: a 31-field descriptor has none
+  d.s0 = n_fields > 31 ? (float*)f[31] : nullptr;
+  d.s1 = n_fields > 32 ? (float*)f[32] : nullptr;
+  d.s2 = n_fields > 33 ? (float*)f[33] : nullptr;
   if (d.lanes < 1) d.lanes = 1;
   d.ept = (d.lanes == 1 && d.size >= (1LL << 20)) ? 4 : 1;
   {
     uintptr_t al = (uintptr_t)d.w | (uintptr_t)d.grad_out | (uintptr_t)d.acc | (uintptr_t)d.vel |
                    (uintptr_t)d.grad[0];
-    d.vec4 = (d.ept == 4 && d.g_cpad == 0 && (al & 15) == 0 &&
+    // solver tensors take the scalar 4-element path: a float4 path that also carries the solver
+    // state compiles to 400 / 722 bytes of spill stores / loads (sm_90a, 64 registers) against
+    // 64 / 74 without it
+    d.vec4 = (d.ept == 4 && d.g_cpad == 0 && (al & 15) == 0 && !(d.flags & UF_SOLVERS) &&
               (d.nparts <= 1 || (d.part_stride & 3) == 0) && (red_off & 3) == 0) ? 1 : 0;
   }
   const int ept = d.ept > 1 ? 1024 : 256 / d.lanes;
@@ -786,7 +862,6 @@ int multi_update_pack(const long long* f, int n_fields, void* out, int tile_begi
   d.n_tiles = (int)((d.size + ept - 1) / ept);
   d.red_off = red_off;
   memcpy(out, &d, sizeof(d));
-  (void)n_fields;
   return d.n_tiles;
 }
 
@@ -828,7 +903,7 @@ void launch_fused_update(float* w, const float* const* grad_ptrs, int nranks, in
                          long long size, int rows, int cols, __nv_bfloat16* lp, int ld,
                          __nv_bfloat16* lp_conv, int taps, int C, int c_pad,
                          uint32_t* const* peer_flags, uint32_t* epoch, int rank, int blocks,
-                         int lp_cpad, int g_cpad, cudaStream_t st) {
+                         int lp_cpad, int g_cpad, float* s0, float* s1, float* s2, cudaStream_t st) {
   GradSources gs{};
   for (int r = 0; r < nranks; ++r) gs.ptr[r] = grad_ptrs[r];
   gs.nranks = nranks; gs.nparts = nparts; gs.part_stride = part_stride; gs.g_cpad = g_cpad;
@@ -840,10 +915,10 @@ void launch_fused_update(float* w, const float* const* grad_ptrs, int nranks, in
   if (blocks <= 0) blocks = fused_update_blocks(size);
   if (peer_flags && nranks > 1)
     launch_k(fused_update_k<true>, blocks, 256, 0, st, w, gs, grad_out, acc, vel, hyper, col_sums, flags,
-                                                  is_bias, size, rows, cols, sh, ps);
+                                                  is_bias, size, rows, cols, sh, ps, s0, s1, s2);
   else
     launch_k(fused_update_k<false>, blocks, 256, 0, st, w, gs, grad_out, acc, vel, hyper, col_sums, flags,
-                                                   is_bias, size, rows, cols, sh, ps);
+                                                   is_bias, size, rows, cols, sh, ps, s0, s1, s2);
 }
 void launch_col_sums(const float* w, float* out, int rows, int cols, int transposed, cudaStream_t st) {
   dim3 block(32, 8);

@@ -4,9 +4,11 @@ Parity: /root/reference/gd.py (GradientDescent :73, GDSoftmax :552, GDTanh :561,
 GDRELU :594, GDStrictRELU :623, GDSigmoid :649):
 ``err_output *= f'(y)``; ``err_input = α·err_output·W + β·err_input``;
 ``gradW = err_outputᵀ·x``; ``gradb = Σ_batch err_output``; then the fused SGD step.
-Extra numpy-only solvers of the reference (adagrad / adadelta / fast, :111,395-419)
-are provided with the *intended* maths (SURVEY §9: the reference's adagrad
-multiplies where it should divide).
+The reference's extra solvers (adagrad / adadelta / fast, :111,395-419, numpy-only
+there) are provided with the *intended* maths (SURVEY §9: the reference's adagrad
+multiplies where it should divide). :func:`solver_step` is their numpy oracle; on
+the GPU they run inside the fused update kernels (csrc/update.cu::step_elem) on
+per-parameter state kept in device memory.
 
 H100 path (kernels/api.py): act-derivative is fused into the producer of the
 two wgmma GEMMs' operand (one elementwise pass that also emits the column sums
@@ -21,6 +23,54 @@ from ..core.memory import Array, reshape
 from . import nn_units
 from .nn_units import (ACT_LINEAR, ACT_TANH, ACT_RELU, ACT_STRICT_RELU,
                        ACT_SIGMOID)
+
+
+# solver state arrays of one parameter tensor, by name (GDCommon.solver_state keys (name, part))
+#   adagrad     h       = sum of squared steps
+#   adadelta    E[dx²]  (running mean of the squared adapted steps)
+#   adadelta_g  E[g²]   (running mean of the squared steps)
+#   fast        f       (fast weights)
+SOLVER_STATE = {"adagrad": ("adagrad",), "adadelta": ("adadelta", "adadelta_g"),
+                "fast": ("fast",)}
+# flag bits of the fused update kernel (GradientDescentBase.update_flags)
+SOLVER_FLAGS = {"adagrad": 32, "adadelta": 64, "fast": 128}
+
+
+def solver_step(weights, gradient, velocity, state, solvers, adagrad_epsilon=1e-8,
+                adadelta_momentum=0.9, adadelta_epsilon=1e-8, fast_learning_rate=0.02,
+                apply_gradient=True, weights_transposed=False):
+    """The solver half of one update, in place on ``weights`` and the ``state`` arrays.
+
+    ``gradient`` is the step after regularisation, accumulation and momentum (it is also what
+    ``velocity`` holds when there is one; the velocity keeps that pre-solver value). Adagrad or
+    adadelta rescale it, ``fast`` decays its fast weights and adds ``fast_learning_rate * velocity``,
+    then ``weights += gradient`` and, for non-transposed weights, ``weights -= f``. ``state`` maps
+    the names of :data:`SOLVER_STATE` to arrays shaped like the weights. Returns the final step.
+    The fused update kernel (csrc/update.cu::step_elem) computes the same in the same order."""
+    if "adagrad" in solvers:
+        h = state["adagrad"]
+        h += gradient ** 2
+        gradient = gradient / numpy.sqrt(h + adagrad_epsilon)
+    if "adadelta" in solvers:
+        eg = state["adadelta_g"]
+        ed = state["adadelta"]
+        rho = adadelta_momentum
+        eg *= rho
+        eg += (1 - rho) * gradient ** 2
+        gradient = gradient * numpy.sqrt(ed + adadelta_epsilon) / \
+            numpy.sqrt(eg + adadelta_epsilon)
+        ed *= rho
+        ed += (1 - rho) * gradient ** 2
+    if "fast" in solvers:
+        f = state["fast"]
+        f *= 0.95
+        if velocity is not None:
+            f += fast_learning_rate * velocity
+    if apply_gradient:
+        weights += gradient
+        if "fast" in solvers and not weights_transposed:
+            weights -= state["fast"]
+    return gradient
 
 
 class GDCommon(nn_units.GradientDescentBase):
@@ -46,6 +96,8 @@ class GDCommon(nn_units.GradientDescentBase):
         self.adadelta_epsilon = kwargs.get("adadelta_epsilon", 1e-8)
         self.adagrad_epsilon = kwargs.get("adagrad_epsilon", 1e-8)
         self.solver_state = {}
+        # marks units built by a version whose update kernels run the solvers (see initialize)
+        self.solvers_on_device = True
 
     @property
     def solvers(self):
@@ -69,19 +121,67 @@ class GDCommon(nn_units.GradientDescentBase):
     def initialize(self, device=None, **kwargs):
         if not self.input or not self.err_output:
             return True
-        if self.extra_solvers:
-            # host-only maths, like the reference (/root/reference/gd.py:111,395-419)
+        if "solvers_on_device" not in self.__dict__:
+            # restored from a snapshot of an earlier version, which sent every unit with an extra
+            # solver (and every RProp unit) to the host by setting force_numpy: that flag did not
+            # come from the user, the unit goes back to the device
+            if self.forced_host_by_solvers():
+                self.force_numpy = False
+            self.solvers_on_device = True
+        if self.extra_solvers and not (self.variant_gradient and self.variant_moment_gradient):
+            # the update kernels implement the default gradient / momentum variants only; the
+            # other variants keep the host maths of the numpy oracle (as before the solvers ran
+            # on the device)
             self.force_numpy = True
         super().initialize(device=device, **kwargs)
-        for s in self.extra_solvers:
-            for part, ref in (("weights", self.weights), ("bias", self.bias)):
-                if ref:
-                    self.solver_state[(s, part)] = numpy.zeros_like(ref.mem)
-                    if s == "adadelta":
-                        self.solver_state[(s + "_g", part)] = numpy.zeros_like(ref.mem)
+        self.init_solver_state()
         if self.extra_solvers and not self.gradient_weights_with_moment:
             raise ValueError("Some of the solvers need moment vectors")
         return None
+
+    def init_solver_state(self):
+        """One :class:`Array` per solver state tensor, kept across re-initialisation. A snapshot
+        may carry the state as plain numpy arrays (the form of earlier versions): their values are
+        adopted."""
+        for s in self.extra_solvers:
+            for part, ref in (("weights", self.weights), ("bias", self.bias)):
+                if not ref:
+                    continue
+                for name in SOLVER_STATE[s]:
+                    old = self.solver_state.get((name, part))
+                    if isinstance(old, Array) and old.size == ref.size:
+                        continue
+                    if isinstance(old, numpy.ndarray) and old.size == ref.size:
+                        arr = Array(old.reshape(ref.shape).astype(ref.dtype))
+                    else:
+                        arr = Array(numpy.zeros_like(ref.mem))
+                    self.solver_state[(name, part)] = arr
+        self.init_vectors(*self.solver_state.values())
+
+    def forced_host_by_solvers(self):
+        """Whether earlier versions forced this unit onto the host because of its solvers."""
+        return bool(self.extra_solvers)
+
+    def solver_flags(self, for_bias=False):
+        f = 0
+        for s in self.extra_solvers:
+            f |= SOLVER_FLAGS[s]
+        return f
+
+    def solver_hyper_values(self):
+        return (self.adagrad_epsilon, self.adadelta_momentum, self.adadelta_epsilon,
+                self.fast_learning_rate) + (0.0,) * 4
+
+    def solver_arrays(self, for_bias=False):
+        """(s0, s1, s2) state of the fused update kernel: s0 adagrad h or adadelta E[dx²],
+        s1 adadelta E[g²], s2 fast f."""
+        part = "bias" if for_bias else "weights"
+        get = lambda name: self.solver_state.get((name, part))  # noqa: E731
+        s0 = get("adagrad") if "adagrad" in self.solvers else (
+            get("adadelta") if "adadelta" in self.solvers else None)
+        s1 = get("adadelta_g") if "adadelta" in self.solvers else None
+        s2 = get("fast") if "fast" in self.solvers else None
+        return s0, s1, s2
 
     # -- numpy oracle -------------------------------------------------------------------
     def moment_use(self, vec_old, grad, moment):
@@ -128,29 +228,14 @@ class GDCommon(nn_units.GradientDescentBase):
             gradient = self.moment_use(vec_old, gradient, moment)
             gradient = -step(vec.mem, gradient, lr, factor_l12, l1_vs_l2,
                              f_ortho, v_trans)
-        if "adagrad" in self.solvers:
-            h = self.solver_state[("adagrad", s)]
-            h += gradient ** 2
-            gradient = gradient / numpy.sqrt(h + self.adagrad_epsilon)
-        if "adadelta" in self.solvers:
-            eg = self.solver_state[("adadelta_g", s)]
-            ed = self.solver_state[("adadelta", s)]
-            rho = self.adadelta_momentum
-            eg *= rho
-            eg += (1 - rho) * gradient ** 2
-            gradient = gradient * numpy.sqrt(ed + self.adadelta_epsilon) / \
-                numpy.sqrt(eg + self.adadelta_epsilon)
-            ed *= rho
-            ed += (1 - rho) * gradient ** 2
-        if "fast" in self.solvers:
-            f = self.solver_state[("fast", s)]
-            f *= 0.95
-            if vec_old:
-                f += self.fast_learning_rate * vec_old.mem
-        if self.apply_gradient:
-            vec.mem += gradient
-            if "fast" in self.solvers and not v_trans:
-                vec.mem -= self.solver_state[("fast", s)]
+        state = {}
+        for (name, part), arr in self.solver_state.items():
+            if part == s:
+                arr.map_write()
+                state[name] = arr.mem
+        solver_step(vec.mem, gradient, vec_old.mem if vec_old else None, state,
+                    self.extra_solvers, self.adagrad_epsilon, self.adadelta_momentum,
+                    self.adadelta_epsilon, self.fast_learning_rate, self.apply_gradient, v_trans)
 
     def on_cuda_forward_shadow(self):
         fu = self.forward_unit

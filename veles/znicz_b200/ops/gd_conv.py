@@ -13,8 +13,6 @@ atomic ``DirectPack`` scatter, /root/reference/gd_conv.py:313-423).
 """
 from __future__ import annotations
 
-import numpy
-
 from . import nn_units
 from .conv import ConvolutionalBase, im2col, col2im, conv_output_size
 from .gd import GDCommon
@@ -34,8 +32,6 @@ class GradientDescentConv(ConvolutionalBase, GDCommon):
     def initialize(self, device=None, **kwargs):
         if not self.input or not self.err_output:
             return True
-        if self.extra_solvers:
-            self.force_numpy = True
         super().initialize(device=device, **kwargs)
         shp = self.input.shape
         if len(shp) == 3:
@@ -55,12 +51,6 @@ class GradientDescentConv(ConvolutionalBase, GDCommon):
                              "kx, ky parameters")
         if self.include_bias and self.bias and self.bias.size != self.n_kernels:
             raise ValueError("Expected bias to match n_kernels")
-        for s in self.extra_solvers:
-            for part, ref in (("weights", self.weights), ("bias", self.bias)):
-                if ref:
-                    self.solver_state[(s, part)] = numpy.zeros_like(ref.mem)
-                    if s == "adadelta":
-                        self.solver_state[(s + "_g", part)] = numpy.zeros_like(ref.mem)
         return None
 
     @property

@@ -39,8 +39,6 @@ class GDDeconv(ConvolutionalBase, GDCommon):
     def initialize(self, device=None, **kwargs):
         if not self.input or not self.err_output or not self.weights:
             return True
-        if self.extra_solvers:
-            self.force_numpy = True
         super().initialize(device=device, **kwargs)
         self.sliding = tuple(self.sliding)
         self.padding = tuple(self.padding)

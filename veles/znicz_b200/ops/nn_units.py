@@ -263,11 +263,16 @@ class GradientDescentBase(AcceleratedUnit, metaclass=MatchingObject):
     MAPPING = set()
     REDUCE_SIZE = 64
     ACT = ACT_LINEAR
-    # layout of the device hyper-parameter vector (csrc/update.cu)
+    # layout of the device hyper-parameter vector (csrc/update.cu::load_step_hyper); the kernel
+    # reads slots from 13 on only when the flags select a solver
     HYPER_FIELDS = ("lr", "wd", "l1_vs_l2", "moment", "acc_alpha", "acc_beta",
                     "gd_alpha", "gd_beta", "factor_ortho", "lr_bias", "wd_bias",
-                    "l1_vs_l2_bias", "moment_bias", "reserved0", "reserved1",
-                    "reserved2")
+                    "l1_vs_l2_bias", "moment_bias", "adagrad_epsilon", "adadelta_rho",
+                    "adadelta_epsilon", "fast_lr", "rprop_increase", "rprop_decrease",
+                    "rprop_min_lr", "rprop_max_lr", "reserved0", "reserved1", "reserved2")
+    # flag bits of the fused update kernel (update_flags)
+    FLAG_APPLY, FLAG_MOMENT, FLAG_ACC, FLAG_ORTHO, FLAG_TRANSPOSED = 1, 2, 4, 8, 16
+    FLAG_ADAGRAD, FLAG_ADADELTA, FLAG_FAST, FLAG_RPROP = 32, 64, 128, 256
 
     def __init__(self, workflow, **kwargs):
         kwargs["view_group"] = kwargs.get("view_group", "TRAINER")
@@ -390,11 +395,26 @@ class GradientDescentBase(AcceleratedUnit, metaclass=MatchingObject):
 
     # -- device hyper-parameters ---------------------------------------------------------
     def hyper_values(self):
-        return (self.learning_rate, self.weights_decay, self.l1_vs_l2,
+        vals = (self.learning_rate, self.weights_decay, self.l1_vs_l2,
                 self.gradient_moment, self.acc_alpha, self.acc_beta,
                 self.gd_alpha, self.gd_beta, self.factor_ortho,
                 self.learning_rate_bias, self.weights_decay_bias,
-                self.l1_vs_l2_bias, self.gradient_moment_bias, 0.0, 0.0, 0.0)
+                self.l1_vs_l2_bias, self.gradient_moment_bias) + \
+            tuple(self.solver_hyper_values())
+        return vals + (0.0,) * (len(self.HYPER_FIELDS) - len(vals))
+
+    # -- solvers beyond SGD + momentum (ops/gd.py, ops/rprop_gd.py) --------------------------
+    def solver_hyper_values(self):
+        """Hyper slots 13-20: adagrad eps, adadelta rho and eps, fast lr, RProp increase,
+        decrease, min and max rate."""
+        return (0.0,) * 8
+
+    def solver_flags(self, for_bias=False):
+        return 0
+
+    def solver_arrays(self, for_bias=False):
+        """Solver state Arrays (s0, s1, s2) the fused update kernel steps with the tensor."""
+        return None, None, None
 
     def sync_hyper(self):
         """Push hyper-parameters to HBM when they changed (outside any graph)."""
@@ -403,12 +423,13 @@ class GradientDescentBase(AcceleratedUnit, metaclass=MatchingObject):
             return
         import torch
         if self.hyper_dev_ is None:
-            self.hyper_dev_ = torch.zeros(16, dtype=torch.float32,
+            n = len(self.HYPER_FIELDS)
+            self.hyper_dev_ = torch.zeros(n, dtype=torch.float32,
                                           device=self.device.torch_device)
             # ring of pinned staging slots (per-iteration LR policies change the values every
             # step while the host runs ahead of the device: a single slot could be rewritten
             # before its queued async copy has executed)
-            self.hyper_host_ = [torch.zeros(16, dtype=torch.float32).pin_memory() for _ in range(8)]
+            self.hyper_host_ = [torch.zeros(n, dtype=torch.float32).pin_memory() for _ in range(8)]
             self.__dict__["hyper_slot_"] = 0
         k = self.__dict__["hyper_slot_"] = (self.__dict__.get("hyper_slot_", 0) + 1) % 8
         host = self.hyper_host_[k]
@@ -438,7 +459,7 @@ class GradientDescentBase(AcceleratedUnit, metaclass=MatchingObject):
             f |= 8
         if self.weights_transposed and not for_bias:
             f |= 16
-        return f
+        return f | self.solver_flags(for_bias)
 
     # -- numpy reference math (/root/reference/nn_units.py:696-719) -----------------------
     def accumulate_gradient_f(self, accumulated_gradient, gradient):
