@@ -544,6 +544,45 @@ void launch_lstm_cell_fwd(const float* z, const float* c_prev, float* c, float* 
   DISPATCH_T(bf16, launch_k(lstm_cell_fwd_k<T>, g, 256, 0, st, z, c_prev, c, gates, (T*)h_out, ldh,
                                                          (T*)h_next, ldn, batch, H));
 }
+// The same cell for the native runtime's tensor-core executor (native/src/engine_cuda.cc), which is
+// held to 1e-4 of its fp32 CPU executor: full-precision expf / tanhf, no gates kept (inference).
+// h_t goes to the output (h_out, nullable) and, as the bf16 parts [hi | hi | lo] of the A-side
+// 3-part split (csrc/split.cu), straight into the h columns of the next step's GEMM operand:
+// xh_next[b * ldn + p * part + j], p = 0, 1, 2 (nullable at the last step).
+__global__ void lstm_cell_split_k(const float* __restrict__ z, const float* __restrict__ c_prev,
+                                  float* __restrict__ c, float* __restrict__ h_out, long long ldh,
+                                  __nv_bfloat16* __restrict__ xh_next, long long ldn, int part,
+                                  int batch, int H) {
+  pdl_entry();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= batch * H) return;
+  const int b = i / H, j = i - b * H;
+  const float* zr = z + (size_t)b * 4 * H;
+  const float ig = 1.f / (1.f + expf(-zr[j]));
+  const float fg = 1.f / (1.f + expf(-zr[H + j]));
+  const float gg = 1.7159f * tanhf(0.6666f * zr[2 * H + j]);
+  const float og = 1.f / (1.f + expf(-zr[3 * H + j]));
+  const float cv = ig * gg + fg * (c_prev ? c_prev[i] : 0.f);
+  const float hv = og * (1.7159f * tanhf(0.6666f * cv));
+  c[i] = cv;
+  if (h_out) h_out[(size_t)b * ldh + j] = hv;
+  if (xh_next) {
+    const __nv_bfloat16 hi = __float2bfloat16_rn(hv);
+    const __nv_bfloat16 lo = __float2bfloat16_rn(hv - __bfloat162float(hi));
+    __nv_bfloat16* o = xh_next + (size_t)b * ldn + j;
+    o[0] = hi;
+    o[part] = hi;
+    o[2 * (size_t)part] = lo;
+  }
+}
+
+void launch_lstm_cell_split(const float* z, const float* c_prev, float* c, float* h_out, long long ldh,
+                            __nv_bfloat16* xh_next, long long ldn, int part, int batch, int H,
+                            cudaStream_t st) {
+  const int g = (batch * H + 255) / 256;
+  launch_k(lstm_cell_split_k, g, 256, 0, st, z, c_prev, c, h_out, ldh, xh_next, ldn, part, batch, H);
+}
+
 void launch_lstm_cell_bwd(const void* err_h, long long lde, const void* dh_rec, long long ldr,
                           const float* dc_next, const float* gates, const float* c,
                           const float* c_prev, float* dc_prev, void* dz, int batch, int H, bool bf16,

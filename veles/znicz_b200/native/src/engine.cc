@@ -113,6 +113,19 @@ Engine::Engine(const std::string& path) {
       auto pd = int_list(d.at("padding")); for (int i = 0; i < 4; ++i) u.pad[i] = pd.at(i);
     } else if (cls == "DropoutForward" || cls == "ZeroFiller") {
       u.kind = "identity";
+    } else if (cls == "LSTMSequence") {
+      u.kind = "lstm";
+      if (wt) throw std::runtime_error(u.cls + ": weights_transposed is not supported (weights must be [4H][I + H])");
+      take_weights();
+      u.hidden = (int)d.at("hidden_size").num;
+      u.return_sequences = d.has("return_sequences") && d.at("return_sequences").b;
+      const int64_t rows = u.weights.shape[0], cols = u.weights.shape[1];
+      if (u.hidden <= 0 || u.hidden >= cols)
+        throw std::runtime_error(u.cls + ": hidden_size " + std::to_string(u.hidden) + " does not fit weights of " +
+                                 std::to_string(cols) + " columns (I + H)");
+      if (rows != 4LL * u.hidden)
+        throw std::runtime_error(u.cls + ": weights have " + std::to_string(rows) + " rows, expected 4 * hidden_size = " +
+                                 std::to_string(4LL * u.hidden));
     } else {
       throw std::runtime_error("unit class " + cls + " is not supported by the native runtime");
     }
@@ -140,6 +153,13 @@ Shape4 Engine::out_shape(const UnitSpec& u, const Shape4& in) const {
   } else if (u.kind == "cutter") {
     o.h = in.h - u.pad[1] - u.pad[3]; o.w = in.w - u.pad[0] - u.pad[2];
     if (o.h <= 0 || o.w <= 0) throw std::runtime_error("cutter: empty output");
+  } else if (u.kind == "lstm") {
+    // a sample is [T][I]: [n, T, I] from python, [n, T * I], or the [T][H] output of an LSTM below
+    const int64_t feat = u.weights.shape[1] - u.hidden, sz = (int64_t)in.h * in.w * in.c;
+    if (sz <= 0 || sz % feat)
+      throw std::runtime_error(u.cls + ": sample size " + std::to_string(sz) + " is not a multiple of " +
+                               std::to_string(feat) + " input features");
+    o.h = u.return_sequences ? (int)(sz / feat) : 1; o.w = 1; o.c = u.hidden;
   }
   return o;
 }
@@ -241,6 +261,33 @@ std::vector<float> Engine::run_cpu(const float* input, const Shape4& in) {
       }
     } else if (u.kind == "act") {
       for (int64_t i = 0; i < s.size(); ++i) nxt[i] = act_code(u.act_code, cur[i], u.factor, (int)(i & 1));
+    } else if (u.kind == "lstm") {
+      // ops/lstm_seq.py numpy_run: z = [x_t | h_{t-1}] W^T + b; i, f, o = sigma, g = A tanh(B z);
+      // c = i g + f c_prev; h = o A tanh(B c); h_{-1} = c_{-1} = 0
+      const int H = u.hidden, K = (int)u.weights.shape[1], I = K - H, T = (int)(s.size() / s.n / I);
+      const float* W = u.weights.data.data();
+      auto sigm = [](double v) { return 1.0 / (1.0 + std::exp(-v)); };
+      auto stanh = [](double v) { return 1.7159 * std::tanh(0.6666 * v); };
+#pragma omp parallel for schedule(static)
+      for (int b = 0; b < s.n; ++b) {
+        std::vector<float> xh(K, 0.f);
+        std::vector<double> z(4 * H), c(H, 0.0);
+        for (int t = 0; t < T; ++t) {
+          std::memcpy(xh.data(), cur.data() + ((size_t)b * T + t) * I, sizeof(float) * I);
+          for (int n = 0; n < 4 * H; ++n) {
+            const float* w = W + (size_t)n * K;
+            double acc = u.include_bias ? u.bias.data[n] : 0.0;
+            for (int k = 0; k < K; ++k) acc += (double)xh[k] * w[k];
+            z[n] = acc;
+          }
+          float* h = u.return_sequences ? &nxt[((size_t)b * T + t) * H] : (t == T - 1 ? &nxt[(size_t)b * H] : nullptr);
+          for (int j = 0; j < H; ++j) {
+            c[j] = sigm(z[j]) * stanh(z[2 * H + j]) + sigm(z[H + j]) * c[j];
+            xh[I + j] = (float)(sigm(z[3 * H + j]) * stanh(c[j]));
+            if (h) h[j] = xh[I + j];
+          }
+        }
+      }
     } else if (u.kind == "cutter") {
       for (int b = 0; b < o.n; ++b) for (int y = 0; y < o.h; ++y) for (int x = 0; x < o.w; ++x)
         std::memcpy(&nxt[(((size_t)b * o.h + y) * o.w + x) * o.c],

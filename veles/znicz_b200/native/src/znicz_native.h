@@ -3,7 +3,8 @@
 //
 // H100-native equivalent of the reference's libZnicz (All2All,
 // All2AllLinear/Tanh/Softmax on libVeles+libSimd, single sample, CPU/NEON), extended to every
-// exportable forward unit (conv, pooling, LRN, activations, cutter, dropout) and to batches.
+// exportable forward unit (conv, pooling, LRN, activations, cutter, dropout, the whole-sequence
+// LSTM) and to batches.
 // Two executors over one unit list: a portable CPU executor (the oracle of the C++ tests) and
 // an sm_90a executor that launches the same hand-written kernels as the training engine
 // (no libtorch, no cuBLAS/cuDNN).
@@ -47,7 +48,7 @@ struct Shape4 { int n = 1, h = 1, w = 1, c = 1; int64_t size() const { return (i
 
 struct UnitSpec {
   std::string cls, uuid;
-  std::string kind;              // all2all | conv | pool | lrn | act | cutter | identity | softmax
+  std::string kind;              // all2all | conv | pool | lrn | act | cutter | identity | softmax | lstm
   Act act = Act::Linear;
   int act_code = 0;              // stand-alone activation kernel code (1..8)
   float factor = 1.f;
@@ -58,6 +59,10 @@ struct UnitSpec {
   int pad[4] = {0, 0, 0, 0};     // left, top, right, bottom
   int pool_mode = 0;             // 0 max, 1 maxabs, 2 avg
   float alpha = 1e-4f, beta = 0.75f, k = 2.f; int n = 5;
+  // lstm: weights [4H][I + H] (gates input, forget, memory, output), bias [4H]; a sample of
+  // h*w*c floats is T = h*w*c / I steps of I features; output [T][H] or the last step's [H]
+  int hidden = 0;
+  bool return_sequences = false;
   std::vector<int> links;
 };
 
