@@ -454,9 +454,63 @@ def test_gather_minibatch_with_channel_padding(ext, src_dt, dst_dt):
     assert torch.equal(dst2, ref)
 
 
+def _softmax64(logits):
+    z = logits - logits.max(axis=1, keepdims=True)
+    e = numpy.exp(z)
+    return e / e.sum(axis=1, keepdims=True)
+
+
+def _eval_state(rows, n_out, err_dtype, confusion):
+    """Evaluator accumulators that already hold earlier minibatches: the kernels must add to them
+    (n_err, confusion) or raise them (max_err_output_sum), never overwrite. err_output is poisoned
+    so that every row, padding rows included, must be written."""
+    rs = numpy.random.RandomState(rows + n_out)
+    st = dict(err=torch.full((rows, n_out), float("nan"), device="cuda").to(err_dtype),
+              n_err=torch.tensor([5, 9], dtype=torch.int32, device="cuda"),
+              mx=torch.tensor([1e-3], device="cuda"),
+              conf=torch.from_numpy(rs.randint(0, 3, (n_out, n_out)).astype(numpy.int32)).cuda()
+              if confusion else None)
+    st["before"] = {k: v.cpu().numpy().copy() for k, v in st.items() if k != "err" and v is not None}
+    return st
+
+
+def _check_against_numpy_evaluator(probs, mi, labels, valid, mean, st, err_dtype):
+    """Device evaluator results == EvaluatorSoftmax.numpy_run fed the device's own probabilities
+    and arg-max: integer results exactly, err_output within the rounding of its storage type."""
+    from veles.znicz_b200.core.memory import Array
+    from veles.znicz_b200.core.workflow import DummyWorkflow
+    from veles.znicz_b200.workflow.evaluator import EvaluatorSoftmax
+    ev = EvaluatorSoftmax(DummyWorkflow(), compute_confusion_matrix=st["conf"] is not None,
+                          mean=mean)
+    ev.output = Array(probs.astype(numpy.float64))
+    ev.max_idx = Array(mi.astype(numpy.int32))
+    ev.labels = Array(labels.astype(numpy.int32))
+    ev.batch_size = valid
+    ev.initialize(device=None)
+    ev.n_err.mem[...] = st["before"]["n_err"]
+    ev.max_err_output_sum.mem[...] = st["before"]["mx"]
+    if st["conf"] is not None:
+        ev.confusion_matrix.mem[...] = st["before"]["conf"]
+    ev.run()
+    assert numpy.array_equal(st["n_err"].cpu().numpy(), ev.n_err.mem)
+    if st["conf"] is not None:
+        assert numpy.array_equal(st["conf"].cpu().numpy(), ev.confusion_matrix.mem)
+    err = st["err"].float().cpu().numpy().astype(numpy.float64)
+    ref = ev.err_output.mem
+    assert numpy.isfinite(err).all()
+    # one rounding of (p - onehot) * mult in fp32 (two ulps of slack), or the bf16 store
+    eps = 2.0 ** -22 if err_dtype == torch.float32 else 2.0 ** -8
+    bad = numpy.abs(err - ref) > eps * numpy.abs(ref)      # zero rows must be exactly zero
+    assert not bad.any(), "err_output differs at %s" % (numpy.argwhere(bad)[:8].tolist(),)
+    # the kernels sum |err| in fp32 before the bf16 store
+    assert abs(float(st["mx"]) - float(ev.max_err_output_sum.mem[0])) <= \
+        1e-5 * float(ev.max_err_output_sum.mem[0])
+
+
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 def test_fc_small_forward_fused_evaluator(ext, dtype):
-    """softmax FC + evaluator in one launch == fc_small_forward followed by evaluate_softmax."""
+    """softmax FC + evaluator in one launch == fc_small_forward followed by evaluate_softmax, and
+    both == a float64 softmax and EvaluatorSoftmax.numpy_run."""
     torch.manual_seed(11)
     dev = "cuda"
     batch, valid, n_in, n_out = 50, 43, 256, 10
@@ -484,6 +538,104 @@ def test_fc_small_forward_fused_evaluator(ext, dtype):
     assert torch.equal(a["n_err"], f["n_err"]) and torch.equal(a["conf"], f["conf"])
     assert torch.allclose(a["err"].float(), f["err"].float(), atol=1e-6 if dtype == torch.float32 else 1e-3)
     assert abs(float(a["mx"]) - float(f["mx"])) < 1e-3
+    logits = x.double().cpu().numpy() @ w.double().cpu().numpy().T + b.double().cpu().numpy()
+    assert numpy.abs(f["out"].cpu().numpy() - _softmax64(logits)).max() < 1e-5
+    assert numpy.array_equal(f["mi"].cpu().numpy(), logits.argmax(axis=1))
+    f["before"] = {"n_err": numpy.zeros(2, numpy.int32), "mx": numpy.zeros(1, numpy.float32),
+                   "conf": numpy.zeros((n_out, n_out), numpy.int32)}
+    _check_against_numpy_evaluator(f["out"].cpu().numpy(), f["mi"].cpu().numpy(),
+                                   labels.cpu().numpy(), valid, True, f, dtype)
+
+
+FC_EVAL_CASES = [(dt, mean, conf, fused) for dt in (torch.float32, torch.bfloat16)
+                 for mean, conf in ((True, True), (False, True), (True, False))
+                 for fused in (True, False)]
+
+
+@pytest.mark.parametrize("dtype,mean,confusion,fused", FC_EVAL_CASES,
+                         ids=["%s-mean%d-conf%d-%s" % (str(d)[6:], m, c, "fused" if f else "alone")
+                              for d, m, c, f in FC_EVAL_CASES])
+def test_fc_small_softmax_evaluator_matches_numpy(ext, dtype, mean, confusion, fused):
+    """The few-output softmax head with its evaluator (fused into the FC launch, or the stand-alone
+    evaluate_softmax_k after it) against a float64 softmax and EvaluatorSoftmax.numpy_run: rows
+    past the batch scalar, labels -1, mean off, no confusion matrix, and exact logit ties, which go
+    to the lowest index as numpy's argmax does."""
+    torch.manual_seed(7)
+    dev = "cuda"
+    rows, valid, n_in, n_out = 64, 37, 192, 10
+    x = torch.randn(rows, n_in, device=dev).to(dtype)
+    w = torch.randn(n_out, n_in, device=dev) * 0.1
+    b = torch.randn(n_out, device=dev) * 0.3
+    w[7] = w[3]                  # classes 3 and 7 have bit-identical logits: a tie in every row
+    b[3] = b[7] = 1.5            # ... that wins in a good share of the rows
+    labels = torch.randint(0, n_out, (rows,), device=dev, dtype=torch.int32)
+    labels[[0, 11, 36]] = -1
+    labels[valid:] = 3           # past the batch scalar: ignored whatever the label says
+    bp = torch.tensor([float(valid), 1.0 / valid if mean else 1.0], device=dev)
+    st = _eval_state(rows, n_out, dtype, confusion)
+    probs = torch.full((rows, n_out), float("nan"), device=dev)
+    mi = torch.full((rows,), -5, dtype=torch.int32, device=dev)
+    if fused:
+        ev = [labels, st["err"], bp, st["n_err"], st["mx"]] + \
+            ([st["conf"]] if confusion else [])
+        ext.fc_small_forward(x, w, b, probs, mi, rows, n_in, n_out, 0, True, ev)
+    else:
+        ext.fc_small_forward(x, w, b, probs, mi, rows, n_in, n_out, 0, True, [])
+        ext.evaluate_softmax(probs, mi, labels, st["err"], bp, st["n_err"], st["conf"], st["mx"])
+    torch.cuda.synchronize()
+    logits = x.double().cpu().numpy() @ w.double().cpu().numpy().T + b.double().cpu().numpy()
+    ref_mi = logits.argmax(axis=1)
+    top2 = numpy.sort(logits, axis=1)[:, -2:]
+    tied = ref_mi == 3
+    assert tied.sum() >= 4 and (logits[tied, 3] == logits[tied, 7]).all()
+    p, m = probs.cpu().numpy(), mi.cpu().numpy()
+    assert (m[tied] == 3).all()
+    # elsewhere the fp32 dot products (error ~1e-6) may only decide a top-two gap below 1e-5
+    clear = ~tied & (top2[:, 1] - top2[:, 0] > 1e-5)
+    assert numpy.array_equal(m[clear], ref_mi[clear])
+    assert (logits[numpy.arange(rows), m] >= top2[:, 1] - 1e-5).all()
+    assert numpy.abs(p - _softmax64(logits)).max() < 1e-5
+    _check_against_numpy_evaluator(p, m, labels.cpu().numpy(), valid, mean, st, dtype)
+
+
+SOFTMAX_ROWS_CASES = [(c, dt) for c in (17, 100, 1000) for dt in (torch.float32, torch.bfloat16)]
+
+
+@pytest.mark.parametrize("cols,dtype", SOFTMAX_ROWS_CASES,
+                         ids=["%d-%s" % (c, str(d)[6:]) for c, d in SOFTMAX_ROWS_CASES])
+def test_softmax_rows_and_evaluator_match_float64(ext, cols, dtype):
+    """softmax_rows_k (the head of every softmax layer with more than 16 outputs, AlexNet's
+    1000-way one included) and evaluate_softmax_k after it, against a float64 softmax and
+    EvaluatorSoftmax.numpy_run. Exact ties are placed in one lane (c, c + 32), across lanes
+    (31 | 32), and between the first and the last column: every one goes to the lowest index."""
+    torch.manual_seed(cols)
+    dev = "cuda"
+    rows, valid = 70, 61
+    logits = (torch.randn(rows, cols, device=dev) * 3.0).to(dtype)
+    ties = [(i, j) for i, j in ((1, 33), (31, 32), (0, cols - 1), (5, 16), (8, 40))
+            if j < cols]
+    for r, (i, j) in enumerate(ties):
+        hi = float(logits[r].float().max()) + 2.0
+        logits[r, i] = logits[r, j] = hi
+    probs = torch.full((rows, cols), float("nan"), device=dev)
+    mi = torch.full((rows,), -5, dtype=torch.int32, device=dev)
+    ext.softmax_rows(logits, probs, mi)
+    labels = torch.randint(0, cols, (rows,), device=dev, dtype=torch.int32)
+    labels[[2, 9]] = -1
+    labels[:3] = mi[:3]          # a few correct predictions
+    bp = torch.tensor([float(valid), 1.0 / valid], device=dev)
+    st = _eval_state(rows, cols, dtype, True)
+    ext.evaluate_softmax(probs, mi, labels, st["err"], bp, st["n_err"], st["conf"], st["mx"])
+    torch.cuda.synchronize()
+    z = logits.double().cpu().numpy()
+    ref_mi = z.argmax(axis=1)
+    p, m = probs.cpu().numpy(), mi.cpu().numpy()
+    assert numpy.array_equal(m, ref_mi)
+    assert [int(m[r]) for r in range(len(ties))] == [i for i, _ in ties]
+    # __expf: a few ulps relative to each probability
+    ref = _softmax64(z)
+    assert (numpy.abs(p - ref) <= 1e-5 * ref + 1e-9).all()
+    _check_against_numpy_evaluator(p, m, labels.cpu().numpy(), valid, True, st, dtype)
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
