@@ -19,6 +19,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from veles.znicz_b200.kernels import load_extension  # noqa: E402
+from veles.znicz_b200.kernels.api import UpdateDesc  # noqa: E402
 
 MAX_BLOCKS = 592
 ADAGRAD, ADADELTA, FAST, RPROP = 32, 64, 128, 256
@@ -32,12 +33,11 @@ def hyper(dev):
                         dtype=torch.float32, device=dev)
 
 
-def fields(w, gout, vel, hyp, colsums, grad, nparts, part_stride, flags, is_bias, rows, cols,
-           lanes, states):
-    p = lambda t: 0 if t is None else int(t.data_ptr())  # noqa: E731
-    return ([p(w), p(gout), 0, p(vel), p(hyp), p(colsums)] + [p(grad)] + [0] * 7 +
-            [int(part_stride), int(w.numel()), int(nparts), 0, int(flags), int(is_bias),
-             int(rows), int(cols), int(lanes), 1, 0, 0, 0, 0, 0, 0, 0] + [p(s) for s in states])
+def desc(w, gout, vel, hyp, colsums, grad, flags, sh, states):
+    return UpdateDesc(w=w, grad=grad, hyper=hyp, nparts=grad.shape[0], part_stride=sh[0] * sh[1],
+                      flags=flags, rows=sh[0], cols=sh[1], is_bias=sh[2], lanes=sh[4],
+                      grad_out=gout, vel=vel, col_sums=colsums, s0=states[0], s1=states[1],
+                      s2=states[2])
 
 
 def main():
@@ -76,13 +76,12 @@ def main():
                   torch.zeros_like(w) if bits & FAST else None]
             flags = 1 | bits | (0 if bits & RPROP else 2) | (8 if cs is not None else 0)
             gr = rank_grads[i]
-            descs.append(fields(w, gout, v, hyp, cs, gr, gr.shape[0], sh[0] * sh[1], flags,
-                                sh[2], sh[0], sh[1], sh[4], st))
+            descs.append(desc(w, gout, v, hyp, cs, gr, flags, sh, st))
             out["w"].append(w)
             out["v"].append(v)
             out["gout"].append(gout)
             out["state"].append(st + [cs])
-        table, tiles, red = ext.multi_update_table(descs, 0)
+        table, tiles, red, _ = ext.multi_update_table(descs, [True] * len(descs), 0)
         out["table"], out["tiles"], out["red"] = table.to(dev), int(tiles), int(red)
         return out
 
@@ -135,13 +134,12 @@ def main():
     pt_ref = build(summed)
     pt_ranks = [build(grads[r]) for r in range(N)]
 
-    def per_tensor(bufs, i, grad_ptrs, peer_flags, epoch_ptr, rank):
+    def per_tensor(bufs, i, grad, grad_ptrs, peer_flags, epoch_ptr, rank):
         sh = shapes[i]
         flags = 1 | sh[5] | (0 if sh[5] & RPROP else 2)          # (no ortho: needs col sums)
-        st = bufs["state"][i]
-        ext.fused_update(bufs["w"][i], grad_ptrs, sh[3], sh[0] * sh[1], bufs["gout"][i], None,
-                         bufs["v"][i], hyp, None, flags, bool(sh[2]), sh[0], sh[1], None, 0, None,
-                         0, 0, 0, peer_flags, epoch_ptr, rank, blocks, 0, 0, st[0], st[1], st[2])
+        ext.fused_update(desc(bufs["w"][i], bufs["gout"][i], bufs["v"][i], hyp, None, grad, flags,
+                              sh, bufs["state"][i]),
+                         grad_ptrs, peer_flags, epoch_ptr, rank, blocks)
     pt_flags = [[torch.zeros(MAX_BLOCKS * 8, dtype=torch.int32, device=dev) for _ in range(N)]
                 for _ in shapes]
     pt_epochs = [[torch.zeros(MAX_BLOCKS, dtype=torch.int32, device=dev) for _ in range(N)]
@@ -149,10 +147,11 @@ def main():
     torch.cuda.synchronize()
     for _step in range(3):
         for i in range(len(shapes)):
-            per_tensor(pt_ref, i, [int(summed[i].data_ptr())], [], 0, 0)
+            per_tensor(pt_ref, i, summed[i], [], [], 0, 0)
             for r in range(N):
                 with torch.cuda.stream(streams[r]):
-                    per_tensor(pt_ranks[r], i, [int(grads[q][i].data_ptr()) for q in range(N)],
+                    per_tensor(pt_ranks[r], i, grads[r][i],
+                               [int(grads[q][i].data_ptr()) for q in range(N)],
                                [int(f.data_ptr()) for f in pt_flags[i]],
                                int(pt_epochs[i][r].data_ptr()), r)
     torch.cuda.synchronize()

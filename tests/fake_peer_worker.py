@@ -21,6 +21,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from veles.znicz_b200.kernels import load_extension  # noqa: E402
+from veles.znicz_b200.kernels.api import UpdateDesc  # noqa: E402
 
 MAX_BLOCKS = 592
 
@@ -29,13 +30,6 @@ def hyper(dev):
     # lr wd l1 moment acc_a acc_b gd_a gd_b ortho lr_b wd_b l1_b moment_b + 3 reserved
     return torch.tensor([0.01, 0.0005, 0.25, 0.9, 0, 0, 0, 1, 0.001, 0.02, 0.0, 0.0, 0.9, 0, 0, 0],
                         dtype=torch.float32, device=dev)
-
-
-def fields(w, vel, hyp, colsums, grad, nparts, part_stride, flags, is_bias, rows, cols, lanes):
-    p = lambda t: 0 if t is None else int(t.data_ptr())
-    return ([p(w), 0, 0, p(vel), p(hyp), p(colsums)] + [p(grad)] + [0] * 7 +
-            [int(part_stride), int(w.numel()), int(nparts), 0, int(flags), int(is_bias),
-             int(rows), int(cols), int(lanes), 1, 0, 0, 0, 0, 0, 0, 0])
 
 
 def main():
@@ -63,9 +57,10 @@ def main():
         for i, sh in enumerate(shapes):
             flags = 1 | 2 | (8 if cs[i] is not None else 0)
             gr = rank_grads[i]
-            descs.append(fields(ws[i], vs[i], hyp, cs[i], gr, gr.shape[0], sh[0] * sh[1], flags,
-                                sh[2], sh[0], sh[1], sh[4]))
-        table, tiles, red = ext.multi_update_table(descs, 0)
+            descs.append(UpdateDesc(w=ws[i], grad=gr, hyper=hyp, nparts=gr.shape[0],
+                                    part_stride=sh[0] * sh[1], flags=flags, rows=sh[0], cols=sh[1],
+                                    is_bias=sh[2], lanes=sh[4], vel=vs[i], col_sums=cs[i]))
+        table, tiles, red, _ = ext.multi_update_table(descs, [True] * len(descs), 0)
         return ws, vs, cs, table.to(dev), int(tiles), int(red)
 
     # ---- oracle: single-GPU kernel fed the (exact) cross-rank sum of the gradients

@@ -13,7 +13,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.mark.gpu
 @pytest.mark.parametrize("n", [2, 4, 8])
 @pytest.mark.parametrize("algo", [0, 1])
-def test_fake_peer_reduce_update_bit_exact(n, algo):
+def test_fake_peer_update_desc_bit_exact(n, algo):
     r = subprocess.run([sys.executable, os.path.join(REPO, "tests", "fake_peer_worker.py"),
                         str(n), str(algo)], capture_output=True, text=True, timeout=300,
                        env=dict(os.environ, PYTHONPATH=REPO))

@@ -3,6 +3,8 @@ import numpy
 import pytest
 import torch
 
+from veles.znicz_b200.kernels.api import UpdateDesc
+
 pytestmark = pytest.mark.gpu
 
 
@@ -195,7 +197,7 @@ def test_conv_fprop_dgrad_wgrad(ext, engine, case):
         assert got == (want_pair, want_tma), (got, want_pair, want_tma)
 
 
-def test_fused_update_matches_reference_formula(ext):
+def test_fused_update_desc_matches_reference_formula(ext):
     """K3/K4 semantics (/root/reference/cuda/gradient_descent.store_output.cu)."""
     torch.manual_seed(4)
     dev = "cuda"
@@ -210,8 +212,9 @@ def test_fused_update_matches_reference_formula(ext):
     w0, acc0, vel0 = w.clone(), acc.clone(), vel.clone()
     lp = torch.zeros(rows, 56, device=dev, dtype=torch.bfloat16)
     gout = torch.zeros(rows, cols, device=dev)
-    ext.fused_update(w, [g.data_ptr()], 3, rows * cols, gout, acc, vel, hyper, cs,
-                     1 | 2 | 4 | 8, False, rows, cols, lp, 56, None, 0, 0, 0, [], 0, 0, 0, 0, 0)
+    ext.fused_update(UpdateDesc(w=w, grad=g, hyper=hyper, nparts=3, part_stride=rows * cols,
+                                flags=1 | 2 | 4 | 8, rows=rows, cols=cols, grad_out=gout, acc=acc,
+                                vel=vel, col_sums=cs, lp=lp, ld=56), [], [], 0, 0, 0)
     torch.cuda.synchronize()
     gs = g.sum(0)
     lr, wd, l1, mom, aa, ab, ga, gb, ortho = [float(v) for v in hyper[:9]]
@@ -227,7 +230,7 @@ def test_fused_update_matches_reference_formula(ext):
     assert _rel(lp[:, :cols], (w0 + gd)) < 1e-2
 
 
-def test_multi_update_matches_per_tensor_update(ext):
+def test_multi_update_desc_matches_per_tensor_update(ext):
     """The whole-network step kernel must be bit-compatible (fixed summation order aside)
     with the per-tensor fused update: weights with ortho + split-K partials, a conv tensor
     with channel-padded gradients and both bf16 shadows, and a bias with 128 partials that
@@ -237,8 +240,6 @@ def test_multi_update_matches_per_tensor_update(ext):
     hyper = torch.tensor([0.1, 0.01, 0.3, 0.9, 0.5, 0.25, 0.75, 0.8, 0.002,
                           0.2, 0.0, 0.0, 0.7, 0, 0, 0], device=dev)
 
-    def P(t):
-        return 0 if t is None else t.data_ptr()
     specs = []
     # (rows, cols, nparts, flags, is_bias, conv(taps, C, c_pad, lp_cpad, g_cpad), lanes)
     specs.append(dict(rows=37, cols=53, nparts=3, flags=1 | 2 | 4 | 8, bias=False, conv=None,
@@ -287,20 +288,23 @@ def test_multi_update_matches_per_tensor_update(ext):
         a, b = two
         if sp["flags"] & 8:
             ext.col_sums(a["w"], a["cs"], rows, cols, False)
-        ext.fused_update(a["w"], [g.data_ptr()], sp["nparts"], rows * gcols, a["gout"], a["acc"],
-                         a["vel"], hyper, a["cs"] if sp["flags"] & 8 else None, sp["flags"],
-                         sp["bias"], rows, cols, a["lp"], ld, a["lp_conv"], taps, C, c_pad,
-                         [], 0, 0, 0, lp_cpad, g_cpad)
-        descs.append([P(b["w"]), P(b["gout"]), P(b["acc"]), P(b["vel"]), P(hyper),
-                      P(b["cs"]) if sp["flags"] & 8 else 0, g.data_ptr(), 0, 0, 0, 0, 0, 0, 0,
-                      rows * gcols, rows * cols, sp["nparts"], g_cpad, sp["flags"],
-                      1 if sp["bias"] else 0, rows, cols, sp["lanes"], 1,
-                      P(b["lp"]), ld, lp_cpad, P(b["lp_conv"]), taps, C, c_pad])
+
+        def desc(t):
+            return UpdateDesc(w=t["w"], grad=g, hyper=hyper, nparts=sp["nparts"],
+                              part_stride=rows * gcols, flags=sp["flags"], rows=rows, cols=cols,
+                              is_bias=int(sp["bias"]), lanes=sp["lanes"], grad_out=t["gout"],
+                              acc=t["acc"], vel=t["vel"],
+                              col_sums=t["cs"] if sp["flags"] & 8 else None, g_cpad=g_cpad,
+                              lp=t["lp"], ld=ld, lp_cpad=lp_cpad, lp_conv=t["lp_conv"], taps=taps,
+                              c=C, c_pad=c_pad)
+        ext.fused_update(desc(a), [], [], 0, 0, 0)
+        descs.append(desc(b))
         ref.append(a)
         new.append(b)
         sp["g"] = g
-    packed, tiles, red = ext.multi_update_table(descs, 0)
-    assert red == sum((d[15] + 3) // 4 * 4 for d in descs)     # 16-byte aligned slots
+    packed, tiles, red, ortho = ext.multi_update_table(descs, [True] * len(descs), 0)
+    assert red == sum((d.w.numel() + 3) // 4 * 4 for d in descs)     # 16-byte aligned slots
+    assert ortho
     table = packed.cuda()
     sync = torch.zeros(2, dtype=torch.int32, device=dev)
     for _ in range(1):
@@ -317,8 +321,7 @@ def test_multi_update_matches_per_tensor_update(ext):
                 assert _rel(b[k].float(), a[k].float()) < 1e-2, (sp["rows"], k)
                 assert float(b[k].float().abs().sum()) > 0
     # disabled tensors must be left alone; a second launch must work (barrier re-arms)
-    descs[0][23] = 0
-    packed, tiles2, _ = ext.multi_update_table(descs, 0)
+    packed, tiles2, _, _ = ext.multi_update_table(descs, [False] + [True] * (len(descs) - 1), 0)
     assert tiles2 == tiles
     table.copy_(packed)
     w_before = new[0]["w"].clone()

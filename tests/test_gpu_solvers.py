@@ -318,7 +318,7 @@ def test_solver_snapshot_resume_continues():
 
 @pytest.mark.parametrize("n", [2, 4, 8])
 @pytest.mark.parametrize("algo", [0, 1])
-def test_fake_peer_solvers_bit_exact(n, algo):
+def test_fake_peer_solvers_update_desc_bit_exact(n, algo):
     """N fake ranks on one GPU (one-shot and two-shot reduction) == the single-GPU kernel fed the
     summed gradient, bit for bit, with every solver bit set; likewise for the per-tensor kernel."""
     r = subprocess.run([sys.executable, os.path.join(REPO, "tests", "fake_peer_solver_worker.py"),

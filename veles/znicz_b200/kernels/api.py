@@ -14,6 +14,7 @@ a shape raises — there is no silent fallback to PyTorch.
 from __future__ import annotations
 
 import contextlib
+from typing import NamedTuple, Optional
 
 import numpy
 import torch
@@ -368,6 +369,36 @@ def _grad_buffer(unit, name, shape):
     return _tmp(unit, name, shape, torch.float32)
 
 
+class UpdateDesc(NamedTuple):
+    """One parameter update, as both update kernels read it (``ext.cpp::parse_desc``). Buffers
+    are the tensors themselves (None: absent); geometry is in elements."""
+    w: torch.Tensor                           # fp32 master weights [rows][cols]
+    grad: torch.Tensor                        # this rank's split-K partials
+    hyper: torch.Tensor                       # GradientDescentBase.HYPER_FIELDS
+    nparts: int
+    part_stride: int                          # elements between two partials
+    flags: int                                # GradientDescentBase.update_flags
+    rows: int
+    cols: int
+    is_bias: int = 0
+    lanes: int = 1                            # threads summing one element's partials (a power of 2)
+    grad_out: Optional[torch.Tensor] = None   # the reduced gradient (RProp: also the previous one)
+    acc: Optional[torch.Tensor] = None
+    vel: Optional[torch.Tensor] = None
+    col_sums: Optional[torch.Tensor] = None   # ortho regulariser
+    s0: Optional[torch.Tensor] = None         # solver state (adagrad / adadelta / fast / RProp)
+    s1: Optional[torch.Tensor] = None
+    s2: Optional[torch.Tensor] = None
+    g_cpad: int = 0                           # > 0: gradient rows are [tap][g_cpad] channel-padded
+    lp: Optional[torch.Tensor] = None         # bf16 shadow [rows][ld], rows [tap][lp_cpad] if lp_cpad
+    ld: int = 0
+    lp_cpad: int = 0
+    lp_conv: Optional[torch.Tensor] = None    # conv dgrad shadow [tap][roundup(rows, 8)][c_pad]
+    taps: int = 0
+    c: int = 0                                # conv input channels
+    c_pad: int = 0
+
+
 def _update(unit, is_bias, grad_buf, nparts, part_stride, rows, cols, g_cpad=0):
     """Fused (cross-GPU reduce +) SGD step for weights or bias of a GD unit."""
     ext = _ext(unit)
@@ -401,12 +432,6 @@ def _update(unit, is_bias, grad_buf, nparts, part_stride, rows, cols, g_cpad=0):
         if fwd is None or not hasattr(fwd, "kx"):
             raise RuntimeError("channel-padded gradients need the forward conv unit")
         taps, c = fwd.kx * fwd.ky, fwd._n_channels     # fp32x wgrad: no bf16 shadows to refresh
-    dp = unit.dp_
-    if dp is not None and dp.symm is not None and step is None:
-        ptrs, flag_ptrs, epoch_ptr, blocks = dp.symm.peers(unit, grad_buf)
-        rank = dp.rank
-    else:
-        ptrs, flag_ptrs, epoch_ptr, blocks, rank = [grad_buf.data_ptr()], [], 0, 0, 0
     wdev = w.dev
     if flags & unit.FLAG_RPROP:
         if not gout:
@@ -416,38 +441,33 @@ def _update(unit, is_bias, grad_buf, nparts, part_stride, rows, cols, g_cpad=0):
         gout.dev_written()
     else:
         gout_dev = gout.dev_out if gout else None
-    acc_dev = acc.dev if acc else None
-    vel_dev = vel.dev if vel else None
     # solver state (adagrad / adadelta / fast / RProp): stepped in the same kernel
     states = [a if a is not None and a else None for a in unit.solver_arrays(for_bias=is_bias)]
     for bit, a in ((unit.FLAG_ADAGRAD | unit.FLAG_ADADELTA | unit.FLAG_RPROP, states[0]),
                    (unit.FLAG_ADADELTA, states[1]), (unit.FLAG_FAST, states[2])):
         if (flags & bit) and a is None:
             raise RuntimeError("%s: solver state missing for flags %#x" % (unit, flags))
-    sdev = [a.dev if a is not None else None for a in states]
+    s0, s1, s2 = [a.dev if a is not None else None for a in states]
+    lanes = 1                        # whole-network kernel: lane groups for small split-K tensors
+    if wdev.numel() <= 16384:
+        while lanes * 2 <= min(32, nparts):
+            lanes *= 2
+    desc = UpdateDesc(w=wdev, grad=grad_buf, hyper=unit.hyper_dev_, nparts=int(nparts),
+                      part_stride=int(part_stride), flags=int(flags), rows=int(rows),
+                      cols=int(cols), is_bias=int(is_bias), lanes=lanes, grad_out=gout_dev,
+                      acc=acc.dev if acc else None, vel=vel.dev if vel else None,
+                      col_sums=colsums, s0=s0, s1=s1, s2=s2, g_cpad=int(g_cpad), lp=lp,
+                      ld=int(ld), lp_cpad=int(cpad_lp), lp_conv=lp_conv, taps=int(taps),
+                      c=int(c), c_pad=int(c_pad))
+    dp = unit.dp_
     if step is not None:
-        # deferred: the whole-network step kernel applies it (ops/fused_step.py)
-        size = wdev.numel()
-        total_parts = nparts * len(ptrs)
-        lanes = 1
-        if size <= 16384:
-            while lanes * 2 <= min(32, total_parts if len(ptrs) == 1 else nparts):
-                lanes *= 2
-        p = lambda t: 0 if t is None else int(t.data_ptr())
-        fields = ([p(wdev), p(gout_dev), p(acc_dev), p(vel_dev), p(unit.hyper_dev_),
-                   p(colsums)] + [int(x) for x in ptrs] + [0] * (8 - len(ptrs)) +
-                  [int(part_stride), int(size), int(nparts), int(g_cpad), int(flags),
-                   1 if is_bias else 0, int(rows), int(cols), lanes, 1,
-                   p(lp), int(ld), int(cpad_lp), p(lp_conv), int(taps), int(c), int(c_pad)] +
-                  [p(t) for t in sdev])
-        step.submit(unit, is_bias, fields,
-                    (wdev, gout_dev, acc_dev, vel_dev, colsums, lp, lp_conv, *sdev, grad_buf),
-                    grad_buf.data_ptr())
+        step.submit(unit, is_bias, desc)    # deferred: the whole-network step (ops/fused_step.py)
     else:
-        ext.fused_update(wdev, ptrs, nparts, part_stride, gout_dev, acc_dev, vel_dev,
-                         unit.hyper_dev_, colsums, flags, is_bias, rows, cols, lp, ld, lp_conv,
-                         taps, c, c_pad, flag_ptrs, epoch_ptr, rank, blocks, cpad_lp, g_cpad,
-                         *sdev)
+        if dp is not None and dp.symm is not None:
+            ptrs, flag_ptrs, epoch_ptr, blocks = dp.symm.peers(unit, grad_buf)
+            ext.fused_update(desc, ptrs, flag_ptrs, epoch_ptr, dp.rank, blocks)
+        else:
+            ext.fused_update(desc, [], [], 0, 0, 0)
         _launch()
         if not is_bias and getattr(fwd, "weights_q_", None) is not None:
             requantize_weights(fwd)

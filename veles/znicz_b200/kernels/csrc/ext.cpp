@@ -6,6 +6,7 @@
 #include <vector>
 #include <cstring>
 #include "host_loader.h"
+#include "update.h"
 
 namespace zn {
 struct ConvGeom { int N, H, W, C, OH, OW, F, KY, KX, SY, SX, PT, PL; };
@@ -39,8 +40,7 @@ void launch_softmax_rows(const void*, bool, float*, int*, int, int, cudaStream_t
 void launch_evaluate_softmax(const float*, const int*, const int*, void*, bool, const float*, int, int, int*, int*, float*, cudaStream_t);
 void launch_evaluate_mse(const void*, const void*, bool, void*, bool, const float*, int, int, const float*, int, float*, float*, cudaStream_t);
 void launch_mse_find_closest(const void*, bool, const float*, const int*, const float*, int, int, int, int*, cudaStream_t);
-int fused_update_blocks(long long size);
-void launch_fused_update(float*, const float* const*, int, int, long long, float*, float*, float*, const float*, const float*, int, int, long long, int, int, __nv_bfloat16*, int, __nv_bfloat16*, int, int, int, uint32_t* const*, uint32_t*, int, int, int, int, float*, float*, float*, cudaStream_t);
+void launch_fused_update(const TensorDesc&, const float* const*, int, uint32_t* const*, uint32_t*, int, int, cudaStream_t);
 void launch_col_sums(const float*, float*, int, int, int, cudaStream_t);
 void launch_lstm_cell_fwd(const float*, const float*, float*, float*, void*, long long, void*, long long, int, int, bool, cudaStream_t);
 void launch_lstm_cell_bwd(const void*, long long, const void*, long long, const float*, const float*, const float*, const float*, float*, void*, int, int, bool, cudaStream_t);
@@ -54,11 +54,9 @@ long long conv_pair_launches();
 long long conv_halo_launches();
 int launch_fc_wgrad_pair(const void*, long long, const void*, long long, float*, long long, int, int, int,
                          cudaStream_t);
-size_t multi_update_desc_size();
 void set_dp_gradient_scale(float);
 float get_dp_gradient_scale();
-int multi_update_max_tensors();
-int multi_update_pack(const long long*, int, void*, int, long long);
+int multi_update_pack(TensorDesc&, int, long long);
 void launch_multi_update(const void*, int, int, int, int, uint32_t* const*, uint32_t*, int, unsigned*, float* const*, long long, int, float* const*, float*, float*, int, int, cudaStream_t);
 void launch_refresh_shadows(const float*, long long, int, int, __nv_bfloat16*, int, __nv_bfloat16*, int, int, int, int, cudaStream_t);
 void launch_gemm_simt(const void*, bool, long long, int, const void*, bool, long long, int, void*, bool, long long, int, int, int, int, const float*, int, float, float, int, long long, cudaStream_t);
@@ -504,83 +502,104 @@ static float* mfptr_or_null(const c10::optional<Tensor>& t) {
   return t->data_ptr<float>();
 }
 
-// grad_ptrs: list of int64 device addresses (one per rank; local first when single GPU)
-void fused_update(Tensor w, std::vector<int64_t> grad_ptrs, int64_t nparts, int64_t part_stride,
-                  c10::optional<Tensor> grad_out, c10::optional<Tensor> acc, c10::optional<Tensor> vel,
-                  Tensor hyper, c10::optional<Tensor> col_sums, int64_t flags, bool is_bias, int64_t rows,
-                  int64_t cols, c10::optional<Tensor> lp, int64_t ld, c10::optional<Tensor> lp_conv,
-                  int64_t taps, int64_t C, int64_t c_pad, std::vector<int64_t> peer_flags,
-                  int64_t epoch_ptr, int64_t rank, int64_t blocks, int64_t lp_cpad, int64_t g_cpad,
-                  c10::optional<Tensor> s0, c10::optional<Tensor> s1, c10::optional<Tensor> s2) {
-  TORCH_CHECK(w.scalar_type() == torch::kFloat32 && w.is_cuda() && w.is_contiguous());
+// One parameter update (kernels/api.py::UpdateDesc), read by attribute name: a missing attribute
+// raises. Every check of the update's inputs is here, for both update kernels.
+static zn::TensorDesc parse_desc(const py::handle& desc) {
+  // a buffer: None or an empty tensor is absent (null)
+  auto buf = [&](const char* name, torch::ScalarType dt) -> Tensor {
+    const py::object o = desc.attr(name);
+    const Tensor t = o.is_none() ? Tensor() : o.cast<Tensor>();
+    if (!t.defined() || t.numel() == 0) return Tensor();
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == dt, "update descriptor: ", name, " must be a CUDA ",
+                dt == torch::kFloat32 ? "float32" : "bfloat16", " tensor");
+    return t;
+  };
+  auto f32 = [&](const char* name) {
+    const Tensor t = buf(name, torch::kFloat32);
+    return t.defined() ? t.data_ptr<float>() : nullptr;
+  };
+  auto bf16 = [&](const char* name) {
+    const Tensor t = buf(name, torch::kBFloat16);
+    return t.defined() ? reinterpret_cast<__nv_bfloat16*>(t.data_ptr()) : nullptr;
+  };
+  auto num = [&](const char* name) { return desc.attr(name).cast<int64_t>(); };
+  const Tensor w = desc.attr("w").cast<Tensor>();
+  TORCH_CHECK(w.scalar_type() == torch::kFloat32 && w.is_cuda() && w.is_contiguous(),
+              "update descriptor: w must be a contiguous CUDA float32 tensor");
+  zn::TensorDesc d{};
+  d.w = w.data_ptr<float>();
+  d.size = w.numel();
+  d.grad = f32("grad");
+  TORCH_CHECK(d.grad, "update descriptor: no gradient");
+  d.grad_out = f32("grad_out"); d.acc = f32("acc"); d.vel = f32("vel"); d.col_sums = f32("col_sums");
+  d.sh.lp = bf16("lp"); d.sh.lp_conv = bf16("lp_conv");
+  d.part_stride = num("part_stride");
+  d.nparts = (int)num("nparts"); d.g_cpad = (int)num("g_cpad"); d.flags = (int)num("flags");
+  d.is_bias = (int)num("is_bias"); d.rows = (int)num("rows"); d.cols = (int)num("cols");
+  d.lanes = (int)num("lanes");
+  d.sh.ld = (int)num("ld"); d.sh.lp_cpad = (int)num("lp_cpad"); d.sh.taps = (int)num("taps");
+  d.sh.C = (int)num("c"); d.sh.c_pad = (int)num("c_pad");
   // solver state (update.cu::step_elem): s0 adagrad h / adadelta E[dx^2] / RProp lrs,
   // s1 adadelta E[g^2], s2 fast f; each one element per weight
-  for (const auto* t : {&s0, &s1, &s2})
-    TORCH_CHECK(!t->has_value() || !(*t)->defined() || (*t)->numel() == 0 || (*t)->numel() == w.numel(),
-                "fused_update: solver state must match the weights");
-  TORCH_CHECK(!(flags & 256) || (mfptr_or_null(grad_out) && mfptr_or_null(s0)),
-              "fused_update: RProp needs grad_out (previous gradient) and the rates");
-  TORCH_CHECK(!(flags & (32 | 64)) || mfptr_or_null(s0), "fused_update: adagrad / adadelta need s0");
-  TORCH_CHECK(!(flags & 64) || mfptr_or_null(s1), "fused_update: adadelta needs s1");
-  TORCH_CHECK(!(flags & 128) || mfptr_or_null(s2), "fused_update: fast needs s2");
+  auto state = [&](const char* name) {
+    const Tensor t = buf(name, torch::kFloat32);
+    TORCH_CHECK(!t.defined() || t.numel() == d.size, "update descriptor: solver state must match the weights");
+    return t.defined() ? t.data_ptr<float>() : nullptr;
+  };
+  d.s0 = state("s0"); d.s1 = state("s1"); d.s2 = state("s2");
+  const int fl = d.flags;
+  TORCH_CHECK(!(fl & 256) || (d.grad_out && d.s0), "update descriptor: RProp needs grad_out (previous gradient) and the rates");
+  TORCH_CHECK(!(fl & (32 | 64)) || d.s0, "update descriptor: adagrad / adadelta need s0");
+  TORCH_CHECK(!(fl & 64) || d.s1, "update descriptor: adadelta needs s1");
+  TORCH_CHECK(!(fl & 128) || d.s2, "update descriptor: fast needs s2");
+  const Tensor hyper = desc.attr("hyper").cast<Tensor>();
   TORCH_CHECK(hyper.is_cuda() && hyper.scalar_type() == torch::kFloat32 &&
-              hyper.numel() >= ((flags & (32 | 64 | 128 | 256)) ? 21 : 13),
-              "fused_update: the hyper vector is too short (solver slots 13-20)");
-  TORCH_CHECK(grad_ptrs.size() >= 1 && grad_ptrs.size() <= 8);
-  const float* gp[8]; uint32_t* fl[8];
+              hyper.numel() >= ((fl & (32 | 64 | 128 | 256)) ? 21 : 13),
+              "update descriptor: the hyper vector is too short (solver slots 13-20)");
+  d.hyper = hyper.data_ptr<float>();
+  return d;
+}
+
+// The per-tensor step. grad_ptrs: every rank's split-K partials (int64 device addresses, rank
+// order) when data-parallel; empty: the descriptor's local gradient.
+void fused_update(py::handle desc, std::vector<int64_t> grad_ptrs, std::vector<int64_t> peer_flags,
+                  int64_t epoch_ptr, int64_t rank, int64_t blocks) {
+  const zn::TensorDesc d = parse_desc(desc);
+  TORCH_CHECK(grad_ptrs.size() <= 8);
+  const float* gp[8] = {d.grad}; uint32_t* fl[8];
   for (size_t i = 0; i < grad_ptrs.size(); ++i) gp[i] = reinterpret_cast<const float*>(grad_ptrs[i]);
-  bool multi = peer_flags.size() == grad_ptrs.size() && grad_ptrs.size() > 1;
+  const int nranks = grad_ptrs.empty() ? 1 : (int)grad_ptrs.size();
+  const bool multi = (int)peer_flags.size() == nranks && nranks > 1;
   if (multi) for (size_t i = 0; i < peer_flags.size(); ++i) fl[i] = reinterpret_cast<uint32_t*>(peer_flags[i]);
-  zn::launch_fused_update(w.data_ptr<float>(), gp, (int)grad_ptrs.size(), (int)nparts, part_stride,
-                          mfptr_or_null(grad_out), mfptr_or_null(acc), mfptr_or_null(vel),
-                          hyper.data_ptr<float>(), fptr_or_null(col_sums), (int)flags, is_bias ? 1 : 0,
-                          w.numel(), (int)rows, (int)cols, bptr_or_null(lp), (int)ld, bptr_or_null(lp_conv),
-                          (int)taps, (int)C, (int)c_pad, multi ? fl : nullptr,
-                          reinterpret_cast<uint32_t*>(epoch_ptr), (int)rank, (int)blocks, (int)lp_cpad,
-                          (int)g_cpad, mfptr_or_null(s0), mfptr_or_null(s1), mfptr_or_null(s2), cur());
+  zn::launch_fused_update(d, gp, nranks, multi ? fl : nullptr, reinterpret_cast<uint32_t*>(epoch_ptr),
+                          (int)rank, (int)blocks, cur());
   kcheck();
 }
-// the form without solver state (plain SGD / momentum / accumulation)
-void fused_update_sgd(Tensor w, std::vector<int64_t> grad_ptrs, int64_t nparts, int64_t part_stride,
-                      c10::optional<Tensor> grad_out, c10::optional<Tensor> acc, c10::optional<Tensor> vel,
-                      Tensor hyper, c10::optional<Tensor> col_sums, int64_t flags, bool is_bias, int64_t rows,
-                      int64_t cols, c10::optional<Tensor> lp, int64_t ld, c10::optional<Tensor> lp_conv,
-                      int64_t taps, int64_t C, int64_t c_pad, std::vector<int64_t> peer_flags,
-                      int64_t epoch_ptr, int64_t rank, int64_t blocks, int64_t lp_cpad, int64_t g_cpad) {
-  fused_update(w, grad_ptrs, nparts, part_stride, grad_out, acc, vel, hyper, col_sums, flags, is_bias, rows,
-               cols, lp, ld, lp_conv, taps, C, c_pad, peer_flags, epoch_ptr, rank, blocks, lp_cpad, g_cpad,
-               c10::nullopt, c10::nullopt, c10::nullopt);
-}
-int64_t update_blocks(int64_t size) { return zn::fused_update_blocks(size); }
 
-// Whole-network step table. Each descriptor is 31 to 34 int64 fields:
-// [w, grad_out, acc, vel, hyper, col_sums, grad[0..7], part_stride, size, nparts, g_cpad, flags,
-//  is_bias, rows, cols, lanes, enabled, lp, ld, lp_cpad, lp_conv, taps, C, c_pad
-//  (, s0, s1, s2: solver state, null when absent)]
-// Returns (packed CPU uint8 tensor [n * desc_size], total_tiles).
-std::tuple<Tensor, int64_t, int64_t> multi_update_table(std::vector<std::vector<int64_t>> descs, int64_t red_base) {
-  const size_t ds = zn::multi_update_desc_size();
-  TORCH_CHECK((int)descs.size() <= zn::multi_update_max_tensors(),
-              "multi_update handles at most ", zn::multi_update_max_tensors(), " tensors per launch");
+// Whole-network step table: one descriptor per tensor, enabled[i] = tensor i is stepped this time.
+// Returns (packed CPU uint8 tensor [n * sizeof(TensorDesc)], total_tiles, end of the reduction
+// buffer, whether a tensor has the ortho regulariser: the kernel's column-sum phase).
+std::tuple<Tensor, int64_t, int64_t, bool> multi_update_table(std::vector<py::object> descs,
+                                                              std::vector<bool> enabled, int64_t red_base) {
+  TORCH_CHECK(descs.size() <= (size_t)zn::MU_MAX_TENSORS,
+              "multi_update handles at most ", zn::MU_MAX_TENSORS, " tensors per launch");
+  TORCH_CHECK(enabled.size() == descs.size(), "multi_update_table: one enabled flag per descriptor");
+  const size_t ds = sizeof(zn::TensorDesc);
   Tensor out = torch::zeros({(int64_t)(descs.size() * ds)}, torch::dtype(torch::kUInt8));
   int tiles = 0;
   long long red = red_base;
+  bool has_ortho = false;
   for (size_t i = 0; i < descs.size(); ++i) {
-    const int nf = (int)descs[i].size();
-    TORCH_CHECK(nf >= 31 && nf <= 34, "descriptor must have 31 to 34 fields");
-    std::vector<long long> f(descs[i].begin(), descs[i].end());
-    const long long fl = f[18];
-    auto has = [&](int k) { return nf > k && f[k] != 0; };
-    TORCH_CHECK(!(fl & 256) || (f[1] != 0 && has(31)), "RProp needs grad_out and the rates (field 31)");
-    TORCH_CHECK(!(fl & (32 | 64)) || has(31), "adagrad / adadelta need state field 31");
-    TORCH_CHECK(!(fl & 64) || has(32), "adadelta needs state field 32");
-    TORCH_CHECK(!(fl & 128) || has(33), "fast needs state field 33");
-    tiles += zn::multi_update_pack(f.data(), nf, out.data_ptr<uint8_t>() + i * ds, tiles, red);
+    zn::TensorDesc d = parse_desc(descs[i]);
+    d.enabled = enabled[i] ? 1 : 0;
+    has_ortho |= (d.flags & 8) && d.col_sums && !d.is_bias;
+    tiles += zn::multi_update_pack(d, tiles, red);
+    std::memcpy(out.data_ptr<uint8_t>() + i * ds, &d, ds);
     // one fp32 slot per element in the cross-GPU reduction buffer; every tensor starts on a
     // 16-byte boundary (the 4-elements-per-thread tile path uses float4 accesses)
-    red += (f[15] + 3) / 4 * 4;
+    red += (d.size + 3) / 4 * 4;
   }
-  return std::make_tuple(out, (int64_t)tiles, (int64_t)red);
+  return std::make_tuple(out, (int64_t)tiles, (int64_t)red, has_ortho);
 }
 void multi_update(Tensor table, int64_t n, int64_t total_tiles, bool has_ortho,
                   std::vector<int64_t> peer_flags, int64_t epoch_ptr, int64_t rank, Tensor gridsync,
@@ -1113,14 +1132,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("lrn_forward", &lrn_forward); m.def("lrn_backward", &lrn_backward);
   m.def("softmax_rows", &softmax_rows); m.def("evaluate_softmax", &evaluate_softmax);
   m.def("evaluate_mse", &evaluate_mse); m.def("mse_find_closest", &mse_find_closest);
-  m.def("fused_update", &fused_update_sgd); m.def("fused_update", &fused_update);
-  m.def("update_blocks", &update_blocks);
+  m.def("fused_update", &fused_update);
   m.def("som_split", &som_split); m.def("split_parts", &split_parts); m.def("split_conv_wt", &split_conv_wt); m.def("som_argmin", &som_argmin);
   m.def("som_gravity_split", &som_gravity_split); m.def("som_apply", &som_apply);
   m.def("multi_update_table", &multi_update_table);
   m.def("set_dp_gradient_scale", [](double s) { zn::set_dp_gradient_scale((float)s); });
   m.def("get_dp_gradient_scale", []() { return (double)zn::get_dp_gradient_scale(); });
-  m.def("multi_update_max_tensors", []() { return (int64_t)zn::multi_update_max_tensors(); }); m.def("multi_update", &multi_update);
+  m.def("multi_update_max_tensors", []() { return (int64_t)zn::MU_MAX_TENSORS; }); m.def("multi_update", &multi_update);
   m.def("col_sums", &col_sums); m.def("refresh_shadows", &refresh_shadows);
   m.def("lstm_fwd_persist", &lstm_fwd_persist); m.def("lstm_bwd_persist", &lstm_bwd_persist);
   m.def("lstm_state_floats", &lstm_state_floats); m.def("lstm_part_floats", &lstm_part_floats); m.def("lstm_unpack_state", &lstm_unpack_state);

@@ -20,25 +20,15 @@
 // Cross-GPU ordering uses per-block flag words in symmetric memory (st.release.sys /
 // ld.acquire.sys), with the epoch counter kept in device memory so CUDA-graph replays work.
 #include "common.cuh"
-#include <string.h>
+#include "update.h"
 
 namespace zn {
 
-struct GradSources {
-  const float* ptr[8];   // per-rank base pointers (ptr[0] = local when nranks == 1)
+// the per-tensor kernel's gradient sources: every rank's split-K partials, summed in rank order
+struct GradPeers {
+  const float* ptr[8];   // ptr[0] = TensorDesc::grad when nranks == 1
   int nranks;
-  int nparts;            // split-K partials per rank
-  long long part_stride; // elements between partials
-  int g_cpad;            // > 0: gradient rows are [tap][g_cpad] channel-padded (first conv layer)
   float gscale;          // multiplies the cross-rank sum (1 / world_size: data-parallel mean)
-};
-
-struct ShadowSpec {
-  __nv_bfloat16* lp;       // [rows][ld] bf16 copy of w (row-major as w), may be null
-  int ld;
-  int lp_cpad;             // > 0: lp rows are [tap][lp_cpad] channel-padded
-  __nv_bfloat16* lp_conv;  // conv dgrad operand [tap][f_pad = roundup(rows, 8)][c_pad], may be null
-  int taps, C, c_pad;
 };
 
 struct PeerSync {
@@ -191,13 +181,54 @@ __device__ __forceinline__ void step_elem(const StepHyper& h, const int flags, c
   }
 }
 
+// bf16 copies of element i (weights [rows][cols], conv weights [f = row][tap][ch]) in the layouts
+// the wgmma GEMM / conv kernels consume
+__device__ __forceinline__ void store_shadows(const ShadowSpec& sh, const int rows, const int cols,
+                                              const long long i, const float wv) {
+  const int r = (int)(i / cols), c = (int)(i % cols);
+  int lc = c;
+  if (sh.lp_cpad > 0) { const int tap = c / sh.C; lc = tap * sh.lp_cpad + (c - tap * sh.C); }
+  if (sh.lp) sh.lp[(size_t)r * sh.ld + lc] = __float2bfloat16_rn(wv);
+  if (sh.lp_conv) {
+    const int tap = c / sh.C, ch = c % sh.C;
+    sh.lp_conv[((size_t)tap * ((rows + 7) & ~7) + r) * sh.c_pad + ch] = __float2bfloat16_rn(wv);
+  }
+}
+
+// The update of element i from its reduced gradient g, shared by both update kernels: every load,
+// step_elem, every store, the bf16 shadows. flags has UF_ORTHO cleared when the tensor has no
+// column sums; h = load_step_hyper(d.hyper, flags, d.is_bias).
+__device__ __forceinline__ void apply_elem(const TensorDesc& d, const StepHyper& h, const int flags,
+                                           const long long i, const float g) {
+  const int rows = d.rows, cols = d.cols;
+  // weights [rows=Y][cols=H] (or stored transposed [H][Y]); col index = input index
+  const float cs = (flags & UF_ORTHO) ? d.col_sums[(flags & UF_TRANSPOSED) ? (int)(i / rows) : (int)(i % cols)] : 0.f;
+  const float prev = (flags & UF_RPROP) ? d.grad_out[i] : 0.f;     // read before it is overwritten
+  if (d.grad_out) d.grad_out[i] = g;
+  float wv = d.w[i];
+  float av = (flags & UF_ACC) && h.acc_beta != 0.f ? d.acc[i] : 0.f;
+  float vv = (flags & UF_MOMENT) ? d.vel[i] : 0.f;
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+  if (flags & UF_SOLVERS) {
+    if (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) s0 = d.s0[i];
+    if (flags & UF_ADADELTA) s1 = d.s1[i];
+    if (flags & UF_FAST) s2 = d.s2[i];
+  }
+  step_elem<true>(h, flags, rows, g, cs, prev, wv, av, vv, s0, s1, s2);
+  if (flags & UF_ACC) d.acc[i] = av;
+  if (flags & UF_MOMENT) d.vel[i] = vv;
+  if (flags & UF_SOLVERS) {
+    if (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) d.s0[i] = s0;
+    if (flags & UF_ADADELTA) d.s1[i] = s1;
+    if (flags & UF_FAST) d.s2[i] = s2;
+  }
+  if (flags & UF_APPLY) d.w[i] = wv;
+  if (d.sh.lp) store_shadows(d.sh, rows, cols, i, wv);
+}
+
+// Per-tensor step (tied weights, engine.fused_step = False): grid-stride over the elements of d.
 template <bool MULTI>
-__global__ void fused_update_k(float* __restrict__ w, GradSources gs, float* __restrict__ grad_out,
-                               float* __restrict__ acc, float* __restrict__ vel,
-                               const float* __restrict__ hyper, const float* __restrict__ col_sums,
-                               int flags, int is_bias, long long size, int rows, int cols,
-                               ShadowSpec sh, PeerSync ps, float* __restrict__ s0p,
-                               float* __restrict__ s1p, float* __restrict__ s2p) {
+__global__ void fused_update_k(const TensorDesc d, const GradPeers gp, PeerSync ps) {
   pdl_entry();
   __shared__ uint32_t s_epoch;
   uint32_t epoch = 0;
@@ -207,61 +238,33 @@ __global__ void fused_update_k(float* __restrict__ w, GradSources gs, float* __r
     epoch = s_epoch;
     peer_barrier(ps, 2 * epoch - 1);   // every rank's gradient is complete and visible
   }
-  if (col_sums == nullptr) flags &= ~UF_ORTHO;
-  const StepHyper h = load_step_hyper(hyper, flags, is_bias);
-  const bool transposed = flags & UF_TRANSPOSED;
+  const int flags = d.col_sums != nullptr ? d.flags : (d.flags & ~UF_ORTHO);
+  const StepHyper h = load_step_hyper(d.hyper, flags, d.is_bias);
 
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < size; i += stride) {
+  for (; i < d.size; i += stride) {
     long long gi = i;
-    if (gs.g_cpad > 0) {
-      const int r_ = (int)(i / cols), c_ = (int)(i % cols);
-      const int tap_ = c_ / sh.C, ch_ = c_ - tap_ * sh.C;
-      gi = ((long long)r_ * sh.taps + tap_) * gs.g_cpad + ch_;
+    if (d.g_cpad > 0) {
+      const int r_ = (int)(i / d.cols), c_ = (int)(i % d.cols);
+      const int tap_ = c_ / d.sh.C, ch_ = c_ - tap_ * d.sh.C;
+      gi = ((long long)r_ * d.sh.taps + tap_) * d.g_cpad + ch_;
     }
     float g = 0.f;
-    for (int r = 0; r < gs.nranks; ++r) {        // fixed rank order => bit-identical replicas
-      const float* base = gs.ptr[r] + gi;
+    for (int r = 0; r < gp.nranks; ++r) {        // fixed rank order => bit-identical replicas
+      const float* base = gp.ptr[r] + gi;
       float g0 = 0.f, g1 = 0.f, g2 = 0.f, g3 = 0.f;
       int p = 0;
-      for (; p + 4 <= gs.nparts; p += 4) {       // 4 loads in flight per rank
-        g0 += base[(long long)(p + 0) * gs.part_stride];
-        g1 += base[(long long)(p + 1) * gs.part_stride];
-        g2 += base[(long long)(p + 2) * gs.part_stride];
-        g3 += base[(long long)(p + 3) * gs.part_stride];
+      for (; p + 4 <= d.nparts; p += 4) {        // 4 loads in flight per rank
+        g0 += base[(long long)(p + 0) * d.part_stride];
+        g1 += base[(long long)(p + 1) * d.part_stride];
+        g2 += base[(long long)(p + 2) * d.part_stride];
+        g3 += base[(long long)(p + 3) * d.part_stride];
       }
-      for (; p < gs.nparts; ++p) g0 += base[(long long)p * gs.part_stride];
+      for (; p < d.nparts; ++p) g0 += base[(long long)p * d.part_stride];
       g += (g0 + g1) + (g2 + g3);
     }
-    g *= gs.gscale;
-    // weights [rows=Y][cols=H] (or stored transposed [H][Y]); col index = input index
-    const float cs = (flags & UF_ORTHO) ? col_sums[transposed ? (int)(i / rows) : (int)(i % cols)] : 0.f;
-    const float prev = (flags & UF_RPROP) ? grad_out[i] : 0.f;
-    if (grad_out) grad_out[i] = g;
-    float wv = w[i];
-    float av = (flags & UF_ACC) && h.acc_beta != 0.f ? acc[i] : 0.f;
-    float vv = (flags & UF_MOMENT) ? vel[i] : 0.f;
-    float s0 = (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) ? s0p[i] : 0.f;
-    float s1 = (flags & UF_ADADELTA) ? s1p[i] : 0.f;
-    float s2 = (flags & UF_FAST) ? s2p[i] : 0.f;
-    step_elem<true>(h, flags, rows, g, cs, prev, wv, av, vv, s0, s1, s2);
-    if (flags & UF_ACC) acc[i] = av;
-    if (flags & UF_MOMENT) vel[i] = vv;
-    if (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) s0p[i] = s0;
-    if (flags & UF_ADADELTA) s1p[i] = s1;
-    if (flags & UF_FAST) s2p[i] = s2;
-    if (flags & UF_APPLY) w[i] = wv;
-    if (sh.lp) {
-      int r = (int)(i / cols), c = (int)(i % cols);
-      int lc = c;
-      if (sh.lp_cpad > 0) { int tap = c / sh.C; lc = tap * sh.lp_cpad + (c - tap * sh.C); }
-      sh.lp[(size_t)r * sh.ld + lc] = __float2bfloat16_rn(wv);
-      if (sh.lp_conv) {
-        int tap = c / sh.C, ch = c % sh.C;      // w[f=r][tap][ch]
-        sh.lp_conv[((size_t)tap * ((rows + 7) & ~7) + r) * sh.c_pad + ch] = __float2bfloat16_rn(wv);
-      }
-    }
+    apply_elem(d, h, flags, i, g * gp.gscale);
   }
   if (MULTI) {
     peer_barrier(ps, 2 * epoch);       // nobody still reads my gradient buffer
@@ -289,17 +292,7 @@ __global__ void refresh_shadows_k(const float* __restrict__ w, long long size, i
   pdl_entry();
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < size; i += stride) {
-    float wv = w[i];
-    int r = (int)(i / cols), c = (int)(i % cols);
-    int lc = c;
-    if (sh.lp_cpad > 0) { int tap = c / sh.C; lc = tap * sh.lp_cpad + (c - tap * sh.C); }
-    if (sh.lp) sh.lp[(size_t)r * sh.ld + lc] = __float2bfloat16_rn(wv);
-    if (sh.lp_conv) {
-      int tap = c / sh.C, ch = c % sh.C;
-      sh.lp_conv[((size_t)tap * ((rows + 7) & ~7) + r) * sh.c_pad + ch] = __float2bfloat16_rn(wv);
-    }
-  }
+  for (; i < size; i += stride) store_shadows(sh, rows, cols, i, w[i]);
 }
 
 
@@ -317,20 +310,6 @@ __global__ void refresh_shadows_k(const float* __restrict__ w, long long size, i
 //            partial count is large and the tensor small), SGD step, bf16 shadows
 //   phase 3  peer barrier "nobody still reads my gradient buffers"
 // ------------------------------------------------------------------------------------------
-struct TensorDesc {
-  float* w; float* grad_out; float* acc; float* vel;
-  const float* hyper; float* col_sums;
-  const float* grad[8];
-  long long part_stride, size;
-  int nparts, g_cpad, flags, is_bias, rows, cols, lanes, enabled;
-  ShadowSpec sh;
-  int tile_begin, n_tiles;
-  int ept;                    // elements per thread (lanes == 1 only): 4 for large tensors
-  int vec4;                   // ept == 4 and every array / stride is 16-byte aligned: float4 path
-  long long red_off;          // offset of this tensor in the cross-GPU reduction buffer
-  float* s0; float* s1; float* s2;   // solver state (step_elem), null when unused
-};
-
 struct GridSync { unsigned* count; unsigned* gen; };
 // half > 0: the reduction buffer is double buffered (slot parity alternates every step), which
 // makes the trailing cross-GPU barrier unnecessary; chunks = launches per step
@@ -355,7 +334,6 @@ struct RedBufs {
   float gscale;             // multiplies the cross-rank gradient sum (1 / world: mean over the
                             // global batch, so N ranks x batch b == one process at batch N * b)
 };
-constexpr int MU_MAX_TENSORS = 48;
 constexpr int MU_MAX_PEER_BLOCKS = 592;     // size of the cross-GPU flag / epoch arrays
 
 __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
@@ -459,7 +437,7 @@ __device__ __forceinline__ void multi_elem4(const TensorDesc& d, const long long
 #pragma unroll
     for (int r = 0; r < 8; ++r) g4 = f4add(g4, v[r]);
   } else {
-    const float* base = d.grad[0] + i0;
+    const float* base = d.grad + i0;
     const long long st = d.part_stride;
     float4 a[8];
 #pragma unroll
@@ -519,17 +497,7 @@ __device__ __forceinline__ void multi_elem4(const TensorDesc& d, const long long
       *reinterpret_cast<uint2*>(sh.lp + (size_t)r * sh.ld + c) = pk;
     } else {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const long long i = i0 + j;
-        const int rj = (int)(i / cols), cj = (int)(i % cols);
-        int lc = cj;
-        if (sh.lp_cpad > 0) { const int tap = cj / sh.C; lc = tap * sh.lp_cpad + (cj - tap * sh.C); }
-        sh.lp[(size_t)rj * sh.ld + lc] = __float2bfloat16_rn(wv[j]);
-        if (sh.lp_conv) {
-          const int tap = cj / sh.C, ch = cj % sh.C;
-          sh.lp_conv[((size_t)tap * ((rows + 7) & ~7) + rj) * sh.c_pad + ch] = __float2bfloat16_rn(wv[j]);
-        }
-      }
+      for (int j = 0; j < 4; ++j) store_shadows(sh, rows, cols, i0 + j, wv[j]);
     }
   }
 }
@@ -594,7 +562,7 @@ __device__ __forceinline__ float multi_grad(const TensorDesc& d, const long long
       const int tap_ = c_ / d.sh.C, ch_ = c_ - tap_ * d.sh.C;
       gi = ((long long)r_ * d.sh.taps + tap_) * d.g_cpad + ch_;
     }
-    const float* base = d.grad[0] + gi;
+    const float* base = d.grad + gi;
     float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f, a4 = 0.f, a5 = 0.f, a6 = 0.f, a7 = 0.f;
     // 8 predicated loads in flight per round (the remainder is not serialised: out-of-range
     // slots load nothing and add 0, the summation order stays fixed)
@@ -622,47 +590,11 @@ template <int MODE>
 __device__ __forceinline__ void multi_apply(const TensorDesc& d, const long long i, const bool valid,
                                             const int lane, const float g, const RedBufs& rb,
                                             long long poff) {
-  const int is_bias = d.is_bias;
   if (!valid || lane != 0) return;
   if (MODE == 1) { rb.ptr[rb.rank][poff + d.red_off + i] = g; return; }
 
   const int flags = d.col_sums != nullptr ? d.flags : (d.flags & ~UF_ORTHO);
-  const StepHyper h = load_step_hyper(d.hyper, flags, is_bias);
-  const bool transposed = flags & UF_TRANSPOSED;
-  const int rows = d.rows, cols = d.cols;
-
-  const float cs = (flags & UF_ORTHO) ? d.col_sums[transposed ? (int)(i / rows) : (int)(i % cols)] : 0.f;
-  const float prev = (flags & UF_RPROP) ? d.grad_out[i] : 0.f;     // read before it is overwritten
-  if (d.grad_out) d.grad_out[i] = g;
-  float wv = d.w[i];
-  float av = (flags & UF_ACC) && h.acc_beta != 0.f ? d.acc[i] : 0.f;
-  float vv = (flags & UF_MOMENT) ? d.vel[i] : 0.f;
-  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
-  if (flags & UF_SOLVERS) {
-    if (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) s0 = d.s0[i];
-    if (flags & UF_ADADELTA) s1 = d.s1[i];
-    if (flags & UF_FAST) s2 = d.s2[i];
-  }
-  step_elem<true>(h, flags, rows, g, cs, prev, wv, av, vv, s0, s1, s2);
-  if (flags & UF_ACC) d.acc[i] = av;
-  if (flags & UF_MOMENT) d.vel[i] = vv;
-  if (flags & UF_SOLVERS) {
-    if (flags & (UF_ADAGRAD | UF_ADADELTA | UF_RPROP)) d.s0[i] = s0;
-    if (flags & UF_ADADELTA) d.s1[i] = s1;
-    if (flags & UF_FAST) d.s2[i] = s2;
-  }
-  if (flags & UF_APPLY) d.w[i] = wv;
-  const ShadowSpec& sh = d.sh;
-  if (sh.lp) {
-    const int r = (int)(i / cols), c = (int)(i % cols);
-    int lc = c;
-    if (sh.lp_cpad > 0) { const int tap = c / sh.C; lc = tap * sh.lp_cpad + (c - tap * sh.C); }
-    sh.lp[(size_t)r * sh.ld + lc] = __float2bfloat16_rn(wv);
-    if (sh.lp_conv) {
-      const int tap = c / sh.C, ch = c % sh.C;
-      sh.lp_conv[((size_t)tap * ((rows + 7) & ~7) + r) * sh.c_pad + ch] = __float2bfloat16_rn(wv);
-    }
-  }
+  apply_elem(d, load_step_hyper(d.hyper, flags, d.is_bias), flags, i, g);
 }
 
 template <int MODE>
@@ -827,30 +759,14 @@ static float g_dp_gscale = 1.f;
 void set_dp_gradient_scale(float s) { g_dp_gscale = s; }
 float get_dp_gradient_scale() { return g_dp_gscale; }
 
-size_t multi_update_desc_size() { return sizeof(TensorDesc); }
-int multi_update_max_tensors() { return MU_MAX_TENSORS; }
-
-// fields: see ext.cpp::multi_update_table. Returns the number of tiles.
-int multi_update_pack(const long long* f, int n_fields, void* out, int tile_begin, long long red_off) {
-  TensorDesc d{};
-  d.w = (float*)f[0]; d.grad_out = (float*)f[1]; d.acc = (float*)f[2]; d.vel = (float*)f[3];
-  d.hyper = (const float*)f[4]; d.col_sums = (float*)f[5];
-  for (int r = 0; r < 8; ++r) d.grad[r] = (const float*)f[6 + r];
-  d.part_stride = f[14]; d.size = f[15];
-  d.nparts = (int)f[16]; d.g_cpad = (int)f[17]; d.flags = (int)f[18]; d.is_bias = (int)f[19];
-  d.rows = (int)f[20]; d.cols = (int)f[21]; d.lanes = (int)f[22]; d.enabled = (int)f[23];
-  d.sh.lp = (__nv_bfloat16*)f[24]; d.sh.ld = (int)f[25]; d.sh.lp_cpad = (int)f[26];
-  d.sh.lp_conv = (__nv_bfloat16*)f[27]; d.sh.taps = (int)f[28]; d.sh.C = (int)f[29];
-  d.sh.c_pad = (int)f[30];
-  // fields 31-33 (solver state) are optional: a 31-field descriptor has none
-  d.s0 = n_fields > 31 ? (float*)f[31] : nullptr;
-  d.s1 = n_fields > 32 ? (float*)f[32] : nullptr;
-  d.s2 = n_fields > 33 ? (float*)f[33] : nullptr;
+// The whole-network kernel's share of d: its tiles (from tile_begin on), element path and slot
+// range in the reduction buffer. Returns the number of tiles.
+int multi_update_pack(TensorDesc& d, int tile_begin, long long red_off) {
   if (d.lanes < 1) d.lanes = 1;
   d.ept = (d.lanes == 1 && d.size >= (1LL << 20)) ? 4 : 1;
   {
     uintptr_t al = (uintptr_t)d.w | (uintptr_t)d.grad_out | (uintptr_t)d.acc | (uintptr_t)d.vel |
-                   (uintptr_t)d.grad[0];
+                   (uintptr_t)d.grad;
     // solver tensors take the scalar 4-element path: a float4 path that also carries the solver
     // state compiles to 400 / 722 bytes of spill stores / loads (sm_90a, 64 registers) against
     // 64 / 74 without it
@@ -861,7 +777,6 @@ int multi_update_pack(const long long* f, int n_fields, void* out, int tile_begi
   d.tile_begin = tile_begin;
   d.n_tiles = (int)((d.size + ept - 1) / ept);
   d.red_off = red_off;
-  memcpy(out, &d, sizeof(d));
   return d.n_tiles;
 }
 
@@ -890,35 +805,24 @@ void launch_multi_update(const void* table, int n, int total_tiles, int has_orth
   launch_k(multi_update_k, blocks, 256, 0, st, (const TensorDesc*)table, n, total_tiles, has_ortho, ps, gs, rb);
 }
 
-int fused_update_blocks(long long size) {
-  long long b = (size + 255) / 256;     // one element per thread up to one CTA per SM
-  if (b < 1) b = 1;
-  if (b > num_sms()) b = num_sms();
-  return (int)b;
-}
-
-void launch_fused_update(float* w, const float* const* grad_ptrs, int nranks, int nparts,
-                         long long part_stride, float* grad_out, float* acc, float* vel,
-                         const float* hyper, const float* col_sums, int flags, int is_bias,
-                         long long size, int rows, int cols, __nv_bfloat16* lp, int ld,
-                         __nv_bfloat16* lp_conv, int taps, int C, int c_pad,
+// grad_ptrs: every rank's split-K partials in rank order (nranks == 1: the local d.grad)
+void launch_fused_update(const TensorDesc& d, const float* const* grad_ptrs, int nranks,
                          uint32_t* const* peer_flags, uint32_t* epoch, int rank, int blocks,
-                         int lp_cpad, int g_cpad, float* s0, float* s1, float* s2, cudaStream_t st) {
-  GradSources gs{};
-  for (int r = 0; r < nranks; ++r) gs.ptr[r] = grad_ptrs[r];
-  gs.nranks = nranks; gs.nparts = nparts; gs.part_stride = part_stride; gs.g_cpad = g_cpad;
-  gs.gscale = g_dp_gscale;
-  ShadowSpec sh{lp, ld, lp_cpad, lp_conv, taps, C, c_pad};
+                         cudaStream_t st) {
+  GradPeers gp{};
+  for (int r = 0; r < nranks; ++r) gp.ptr[r] = grad_ptrs[r];
+  gp.nranks = nranks; gp.gscale = g_dp_gscale;
   PeerSync ps{};
   ps.rank = rank; ps.nranks = nranks; ps.epoch = epoch;
   if (peer_flags) for (int r = 0; r < nranks; ++r) ps.flags[r] = peer_flags[r];
-  if (blocks <= 0) blocks = fused_update_blocks(size);
+  if (blocks <= 0) {          // one element per thread up to one CTA per SM
+    const long long b = (d.size + 255) / 256;
+    blocks = b < 1 ? 1 : (b > num_sms() ? num_sms() : (int)b);
+  }
   if (peer_flags && nranks > 1)
-    launch_k(fused_update_k<true>, blocks, 256, 0, st, w, gs, grad_out, acc, vel, hyper, col_sums, flags,
-                                                  is_bias, size, rows, cols, sh, ps, s0, s1, s2);
+    launch_k(fused_update_k<true>, blocks, 256, 0, st, d, gp, ps);
   else
-    launch_k(fused_update_k<false>, blocks, 256, 0, st, w, gs, grad_out, acc, vel, hyper, col_sums, flags,
-                                                   is_bias, size, rows, cols, sh, ps, s0, s1, s2);
+    launch_k(fused_update_k<false>, blocks, 256, 0, st, d, gp, ps);
 }
 void launch_col_sums(const float* w, float* out, int rows, int cols, int transposed, cudaStream_t st) {
   dim3 block(32, 8);

@@ -21,12 +21,13 @@ import torch
 from ..kernels import api
 
 
-def _ptr(t):
-    return 0 if t is None else int(t.data_ptr())
+def _desc_key(desc):
+    """What the packed table holds of an ``api.UpdateDesc``: buffer addresses and the scalars."""
+    return tuple(v.data_ptr() if isinstance(v, torch.Tensor) else v for v in desc)
 
 
 class _Entry(object):
-    __slots__ = ("unit", "is_bias", "fields", "keep", "touched", "grad_ptr")
+    __slots__ = ("unit", "is_bias", "desc", "touched")
 
 
 class FusedStep(object):
@@ -94,7 +95,9 @@ class FusedStep(object):
         return {id(u) for us in owners.values() if len(us) > 1 for u in us}
 
     # -- registration (called by api._update in deferred mode) -----------------------------------
-    def submit(self, unit, is_bias, fields, keep, grad_ptr):
+    def submit(self, unit, is_bias, desc):
+        """Step ``desc`` (an ``api.UpdateDesc``, which also keeps its buffers alive) in the next
+        flush."""
         key = (id(unit), bool(is_bias))
         e = self.index.get(key)
         if e is None:
@@ -104,24 +107,22 @@ class FusedStep(object):
             e.unit, e.is_bias = unit, bool(is_bias)
             self.index[key] = e
             self.entries.append(e)
-            e.fields = None
-        if e.fields != fields:
-            if e.fields is not None and torch.cuda.is_current_stream_capturing():
+            e.desc = None
+        if e.desc is None or _desc_key(e.desc) != _desc_key(desc):
+            if e.desc is not None and torch.cuda.is_current_stream_capturing():
                 raise RuntimeError("FusedStep: %s changed buffers during graph capture" % unit)
-            e.fields = list(fields)
             self.dirty = True
-        e.keep = keep
-        e.grad_ptr = grad_ptr
+        e.desc = desc
         e.touched = True
 
     def refresh_flags(self, unit):
         """Host-side hook (GD ``cuda_prepare``): flags are baked into the table."""
         for is_bias in (False, True):
             e = self.index.get((id(unit), is_bias))
-            if e is not None and e.fields is not None:
+            if e is not None and e.desc is not None:
                 f = unit.update_flags(for_bias=is_bias)
-                if e.fields[18] != f:
-                    e.fields[18] = f
+                if e.desc.flags != f:
+                    e.desc = e.desc._replace(flags=f)
                     self.dirty = True
         if self.dirty and self.table is not None and not torch.cuda.is_current_stream_capturing():
             self._upload()
@@ -131,22 +132,18 @@ class FusedStep(object):
         are split over several launches."""
         ext = self.device.ext
         cap = int(ext.multi_update_max_tensors())
-        descs = []
-        for e in self.entries:
-            f = list(e.fields)
-            f[23] = 1 if e.touched else 0
-            descs.append(f)
+        descs = [e.desc for e in self.entries]
+        enabled = [bool(e.touched) for e in self.entries]
         self.chunks = []
         red = 0
         for i in range(0, len(descs), cap):
             part = descs[i:i + cap]
-            packed, tiles, red = ext.multi_update_table(part, red)
+            packed, tiles, red, ortho = ext.multi_update_table(part, enabled[i:i + cap], red)
             old = self.tables[len(self.chunks)] if len(self.chunks) < len(self.tables) else None
             if old is None or old.numel() != packed.numel():
                 old = torch.empty(packed.numel(), dtype=torch.uint8,
                                   device=self.device.torch_device)
             old.copy_(packed)
-            ortho = any((f[18] & 8) and f[5] and not f[19] for f in part)
             self.chunks.append((old, len(part), int(tiles), ortho))
         self.tables = [c[0] for c in self.chunks]
         self.table = self.tables[0] if self.tables else None
@@ -165,7 +162,7 @@ class FusedStep(object):
                 "fused_step_red", 2 * int(red), with_multicast=True)
             self.red_numel = int(red)
             self._pick_algo(symm, int(red))
-        self.enabled = [bool(e.touched) for e in self.entries]
+        self.enabled = enabled
         self.dirty = False
 
     def _pick_algo(self, symm, numel):
@@ -224,7 +221,7 @@ class FusedStep(object):
             import torch.distributed as dist
             for e in self.entries:
                 if e.touched:
-                    dist.all_reduce(e.keep[-1], op=dist.ReduceOp.SUM)
+                    dist.all_reduce(e.desc.grad, op=dist.ReduceOp.SUM)
         for ci, (table, n, tiles, ortho) in enumerate(self.chunks):
             flags, epoch = self.sync[ci] if self.sync else (self.flag_ptrs, self.epoch_ptr)
             self.device.ext.multi_update(table, n, tiles, ortho, flags, epoch,
