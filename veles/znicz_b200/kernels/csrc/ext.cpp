@@ -52,6 +52,8 @@ int launch_gemm_pair(const void*, long long, const void*, long long, void*, int,
 long long im2col_tma_launches();
 long long conv_pair_launches();
 long long conv_halo_launches();
+long long augment_launches();
+void launch_augment_minibatch(const uint8_t*, long long, const int*, const int*, const int*, const float*, void*, void*, bool, const int*, int*, int, int, int, int, int, int, cudaStream_t);
 int launch_fc_wgrad_pair(const void*, long long, const void*, long long, float*, long long, int, int, int,
                          cudaStream_t);
 void set_dp_gradient_scale(float);
@@ -206,6 +208,58 @@ void gather_minibatch(Tensor src, c10::optional<Tensor> labels_src, Tensor hdr, 
   int* ld = (labels_dst.has_value() && labels_dst->defined()) ? labels_dst->data_ptr<int>() : nullptr;
   zn::launch_gather_minibatch(src.data_ptr(), is_bf16(src), ls, hdr.data_ptr<int>(), dst.data_ptr(),
                               is_bf16(dst), ld, (int)dst.size(0), row, pad, (int)C, 8, cur());
+  kcheck();
+}
+// ImageNet augmentation (csrc/augment.cu): crop at params[r] = (y0, x0, flip), mirror, subtract the
+// mean, convert; rows >= hdr[0] zero. src = uint8 [rows][sy][sx][C] gathered through idx (a dataset
+// resident in HBM) or read in order (streamed rows); labels only with idx.
+void augment_minibatch(Tensor src, Tensor hdr, c10::optional<Tensor> idx, Tensor params,
+                       c10::optional<Tensor> mean, Tensor dst, c10::optional<Tensor> labels_src,
+                       c10::optional<Tensor> labels_dst, c10::optional<Tensor> dst_pad) {
+  TORCH_CHECK(src.is_cuda() && src.is_contiguous() && src.scalar_type() == torch::kUInt8 && src.dim() == 4,
+              "augment_minibatch: src must be a contiguous uint8 [rows][sy][sx][C] device tensor");
+  chk(dst, "dst");
+  TORCH_CHECK(dst.scalar_type() != torch::kInt32 && dst.dim() == 4, "dst must be fp32 or bf16 [n][cy][cx][C]");
+  const int max_rows = (int)dst.size(0), cy = (int)dst.size(1), cx = (int)dst.size(2), C = (int)dst.size(3);
+  const int sy = (int)src.size(1), sx = (int)src.size(2);
+  TORCH_CHECK(src.size(3) == C && cy <= sy && cx <= sx && cy >= 1 && cx >= 1, "augment_minibatch: crop ",
+              cy, "x", cx, "x", C, " does not fit the samples ", sy, "x", sx, "x", src.size(3));
+  chk(hdr, "hdr"); chk(params, "params");
+  TORCH_CHECK(hdr.scalar_type() == torch::kInt32 && hdr.numel() >= 1, "hdr must be int32");
+  TORCH_CHECK(params.scalar_type() == torch::kInt32 && params.numel() >= 3LL * max_rows, "params must be int32 [n][3]");
+  const int* ip = nullptr;
+  if (idx.has_value() && idx->defined()) {
+    chk(*idx, "idx");
+    TORCH_CHECK(idx->scalar_type() == torch::kInt32 && idx->numel() >= max_rows, "idx must be int32 [n]");
+    ip = idx->data_ptr<int>();
+  } else {
+    TORCH_CHECK(src.size(0) >= max_rows, "streamed rows: src must hold one row per output row");
+  }
+  const float* mp = nullptr;
+  if (mean.has_value() && mean->defined()) {
+    chk(*mean, "mean");
+    TORCH_CHECK(mean->scalar_type() == torch::kFloat32 && mean->numel() == (int64_t)sy * sx * C,
+                "mean must be fp32 [sy][sx][C]");
+    mp = mean->data_ptr<float>();
+  }
+  const bool has_ls = labels_src.has_value() && labels_src->defined();
+  const bool has_ld = labels_dst.has_value() && labels_dst->defined();
+  TORCH_CHECK(has_ls == has_ld && (!has_ld || ip), "labels need labels_src, labels_dst and idx");
+  if (has_ld) {
+    chk(*labels_src, "labels_src"); chk(*labels_dst, "labels_dst");
+    TORCH_CHECK(labels_src->scalar_type() == torch::kInt32 && labels_src->numel() >= src.size(0) &&
+                labels_dst->scalar_type() == torch::kInt32 && labels_dst->numel() >= max_rows, "labels: int32");
+  }
+  void* pad = nullptr;
+  if (dst_pad.has_value() && dst_pad->defined()) {
+    chk(*dst_pad, "dst_pad"); same_dt(dst, *dst_pad);
+    TORCH_CHECK(C < 8 && dst_pad->numel() == (int64_t)max_rows * cy * cx * 8, "padded minibatch must be [n][cy][cx][8]");
+    pad = dst_pad->data_ptr();
+  }
+  zn::launch_augment_minibatch(src.data_ptr<uint8_t>(), src.size(0), hdr.data_ptr<int>(), ip,
+                               params.data_ptr<int>(), mp, dst.data_ptr(), pad, is_bf16(dst),
+                               has_ls ? labels_src->data_ptr<int>() : nullptr,
+                               has_ld ? labels_dst->data_ptr<int>() : nullptr, max_rows, sy, sx, C, cy, cx, cur());
   kcheck();
 }
 // dst (device) <- src (pinned host tensor), by a kernel that reads the host memory (see
@@ -1084,17 +1138,23 @@ void som_update(Tensor x, Tensor w, Tensor coords, Tensor argmins, double sigma,
 // slot the H2D copy reads - converted to bf16 on the fly when the device-side minibatch is bf16,
 // so only half the bytes cross PCIe and no cast kernel runs - synchronously or one step ahead on
 // the prefetch pool.
+// A uint8 src with a uint8 dst is the raw-bytes mode: rows are copied as they are.
 static znhost::GatherJob make_gather_job(const Tensor& src, const Tensor& idx, const Tensor& dst, int64_t n) {
   TORCH_CHECK(!src.is_cuda() && !idx.is_cuda() && !dst.is_cuda(), "host tensors expected");
   TORCH_CHECK(src.is_contiguous() && dst.is_contiguous() && idx.is_contiguous());
-  TORCH_CHECK(src.scalar_type() == torch::kFloat32 && idx.scalar_type() == torch::kInt32);
+  TORCH_CHECK(idx.scalar_type() == torch::kInt32, "idx must be int32");
+  const bool raw = src.scalar_type() == torch::kUInt8;
   const bool to_bf16 = dst.scalar_type() == torch::kBFloat16;
-  TORCH_CHECK(to_bf16 || dst.scalar_type() == torch::kFloat32, "dst must be fp32 or bf16");
+  TORCH_CHECK(raw ? dst.scalar_type() == torch::kUInt8
+                  : src.scalar_type() == torch::kFloat32 && (to_bf16 || dst.scalar_type() == torch::kFloat32),
+              "src must be fp32 (dst fp32 or bf16) or uint8 (dst uint8)");
+  TORCH_CHECK(src.dim() >= 1 && dst.dim() >= 1, "src and dst need a row dimension");
   znhost::GatherJob j;
   j.rows = src.size(0); j.row = src.numel() / std::max<int64_t>(j.rows, 1);
   j.cap = dst.size(0); j.n = n;
   TORCH_CHECK(n >= 0 && n <= j.cap && n <= idx.numel() && dst.numel() == j.cap * j.row, "shape mismatch");
-  j.src = src.data_ptr<float>(); j.idx = idx.data_ptr<int>(); j.dst = dst.data_ptr(); j.to_bf16 = to_bf16;
+  TORCH_CHECK(n == 0 || j.rows > 0, "empty src");
+  j.src = src.data_ptr(); j.idx = idx.data_ptr<int>(); j.dst = dst.data_ptr(); j.to_bf16 = to_bf16; j.raw = raw;
   return j;
 }
 void host_gather_rows(Tensor src, Tensor idx, Tensor dst, int64_t n) {
@@ -1116,6 +1176,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mul_backward", &mul_backward); m.def("axpby_2d", &axpby_2d); m.def("crop_nhwc", &crop_nhwc);
   m.def("gather_rows", &gather_rows); m.def("gather_labels", &gather_labels);
   m.def("gather_minibatch", &gather_minibatch);
+  m.def("augment_minibatch", &augment_minibatch);
+  m.def("augment_launches", []() { return (int64_t)zn::augment_launches(); });
   m.def("swap01_2d", &swap01_2d); m.def("device_copy", &device_copy); m.def("metric_reduce", &metric_reduce);
   m.def("space_to_depth", &space_to_depth); m.def("s2d_pack_weights", &s2d_pack_weights); m.def("s2d_unpack_grad", &s2d_unpack_grad);
   m.def("stream_ring_create", &stream_ring_create); m.def("stream_ring_destroy", &stream_ring_destroy);

@@ -1,6 +1,7 @@
 // Host-side minibatch assembly for streaming loaders (dataset in host memory).
 //
-//   gather_rows()      rows by index -> a (pinned) staging buffer, fp32 -> bf16 on the fly
+//   gather_rows()      rows by index -> a (pinned) staging buffer, fp32 -> bf16 on the fly, or
+//                      raw bytes as they are (uint8 ImageNet samples, augmented on the device)
 //   HostPrefetcher     a small persistent worker pool that assembles the NEXT minibatch into the
 //                      next pinned slot while the current step is being enqueued / executed, so
 //                      the training loop never waits for the 0.6-1.2 MB gather (the reference's
@@ -33,22 +34,24 @@ inline void convert_row_bf16(const uint32_t* __restrict__ iu, uint16_t* __restri
 }
 
 struct GatherJob {
-  const float* src = nullptr; int64_t rows = 0, row = 0;   // dataset [rows][row] fp32
+  const void* src = nullptr; int64_t rows = 0, row = 0;    // dataset [rows][row] fp32 (uint8 if raw)
   const int* idx = nullptr;                                // n valid indices
   void* dst = nullptr; int64_t n = 0, cap = 0;             // staging [cap][row], rows >= n zeroed
   bool to_bf16 = false;
+  bool raw = false;                                        // copy the bytes as they are
 };
 
 inline void gather_range(const GatherJob& j, int64_t b, int64_t e) {
-  const size_t esz = j.to_bf16 ? 2 : 4;
+  const size_t isz = j.raw ? 1 : 4;
+  const size_t esz = j.raw ? 1 : (j.to_bf16 ? 2 : 4);
   uint8_t* dp = reinterpret_cast<uint8_t*>(j.dst);
   for (int64_t r = b; r < e; ++r) {
     uint8_t* out = dp + (size_t)r * j.row * esz;
     if (r >= j.n) { memset(out, 0, (size_t)j.row * esz); continue; }
     int64_t k = j.idx[r];
     k = k < 0 ? 0 : (k >= j.rows ? j.rows - 1 : k);
-    const float* in = j.src + (size_t)k * j.row;
-    if (!j.to_bf16) memcpy(out, in, (size_t)j.row * 4);
+    const uint8_t* in = reinterpret_cast<const uint8_t*>(j.src) + (size_t)k * j.row * isz;
+    if (!j.to_bf16) memcpy(out, in, (size_t)j.row * esz);
     else convert_row_bf16(reinterpret_cast<const uint32_t*>(in), reinterpret_cast<uint16_t*>(out), j.row);
   }
 }

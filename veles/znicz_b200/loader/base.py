@@ -66,6 +66,22 @@ class LoaderError(Exception):
     pass
 
 
+def channel_pad_target(md):
+    """The channel-padded copy ``[n][h][w][8]`` of the minibatch that a first conv layer with
+    C < 8 asks for (``pad_request_`` on the Array, kernels/api.py::conv_forward), allocated on
+    first use, so the loader's device kernel writes it with the minibatch; None when nobody asked."""
+    cp = md.__dict__.get("pad_request_")
+    if not cp or md.devmem.dim() != 4 or md.devmem.shape[3] >= 8:
+        return None
+    pad = md.__dict__.get("padded_dev_")
+    shape = tuple(md.devmem.shape[:3]) + (8,)
+    if pad is None or tuple(pad.shape) != shape or pad.dtype != md.devmem.dtype:
+        import torch
+        pad = torch.zeros(shape, dtype=md.devmem.dtype, device=md.devmem.device)
+        md.__dict__["padded_dev_"] = pad
+    return pad
+
+
 class Loader(AcceleratedUnit, metaclass=UserLoaderRegistry):
     """Serves minibatches. Subclasses implement ``load_data`` (set class_lengths),
     ``create_minibatch_data`` and ``fill_minibatch``."""
@@ -338,6 +354,17 @@ class Loader(AcceleratedUnit, metaclass=UserLoaderRegistry):
             prof[1] += t2 - t1     # bookkeeping + minibatch assembly on the host
             prof[2] += t3 - t2     # H2D enqueue (+ gather launch)
             prof[3] += 1
+
+    def peek_next_indices(self):
+        """(start, count) of the slice of ``shuffled_indices`` the *next* ``run()`` will serve, or
+        None when that run starts a new epoch (the train part is reshuffled first, so its indices
+        are not known yet). Pure function of the loader state after a ``run()``."""
+        start = self.global_offset
+        if start <= 0 or start >= self.total_samples:
+            return None
+        cls = self.class_index_by_offset(start)
+        n = int(min(self.max_minibatch_size, self.class_end_offsets[cls] - start))
+        return (start, n) if n > 0 else None
 
     def _update_flags(self):
         last_mb = self.global_offset == self.class_end_offsets[self.minibatch_class]

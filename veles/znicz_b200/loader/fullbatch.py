@@ -24,7 +24,7 @@ from ..core.config import root
 from ..core.accelerated_units import host_dtype
 from ..core.memory import Array
 from .base import (Loader, LoaderMSEMixin, LoaderWithValidationRatio, TEST, VALID,
-                   TRAIN, LoaderError)
+                   TRAIN, LoaderError, channel_pad_target)
 
 
 def _pull_ok(ext):
@@ -325,17 +325,6 @@ class FullBatchLoader(Loader, LoaderWithValidationRatio):
         else:
             pk["slots"][i]["event"].synchronize()
 
-    def peek_next_indices(self):
-        """(start, count) of the slice of ``shuffled_indices`` the *next* ``run()`` will serve, or
-        None when that run starts a new epoch (the train part is reshuffled first, so its indices
-        are not known yet). Pure function of the loader state after a ``run()``."""
-        start = self.global_offset
-        if start <= 0 or start >= self.total_samples:
-            return None
-        cls = self.class_index_by_offset(start)
-        n = int(min(self.max_minibatch_size, self.class_end_offsets[cls] - start))
-        return (start, n) if n > 0 else None
-
     def _prefetch_next(self):
         """Start assembling the following minibatch (same epoch only: its indices are already
         fixed in ``shuffled_indices``) into the next pinned slot on the native worker pool."""
@@ -406,16 +395,8 @@ class FullBatchLoader(Loader, LoaderWithValidationRatio):
             # a first conv layer with C % 8 != 0 asks for a channel-padded copy
             # (``pad_request_`` on the Array, kernels/api.py::conv_forward): produce it here
             md = self.minibatch_data
-            pad, c = None, 0
-            cp = md.__dict__.get("pad_request_")
-            if cp and md.devmem.dim() == 4 and md.devmem.shape[3] < 8:
-                pad = md.__dict__.get("padded_dev_")
-                shape = tuple(md.devmem.shape[:3]) + (8,)
-                if pad is None or tuple(pad.shape) != shape or pad.dtype != md.devmem.dtype:
-                    import torch
-                    pad = torch.zeros(shape, dtype=md.devmem.dtype, device=md.devmem.device)
-                    md.__dict__["padded_dev_"] = pad
-                c = int(md.devmem.shape[3])
+            pad = channel_pad_target(md)
+            c = int(md.devmem.shape[3]) if pad is not None else 0
             ext.gather_minibatch(
                 self.original_data.devmem,
                 self._mapped_original_labels.devmem if labels else None,
