@@ -2,7 +2,8 @@
 hand-rolled synchronisation protocol of the repo on sizes a sanitizer run can finish -
 gemm_umma_k (mbarrier ring, TMA + LDGSTS producers, wgmma), gemm_pair_k (producer / MMA
 warpgroups, TMA-store epilogue), lstm kernels (barrier.cluster), multi_update_k (grid barrier;
-fake-peer flag protocol with 2 ranks sharing the GPU), fc_small, pooling / LRN / evaluator."""
+fake-peer flag protocol with 2 ranks sharing the GPU), fc_small, pooling / LRN / evaluator,
+rbm_sample_k / rbm_apply_k (ragged shapes: partial batch, partial transpose tiles)."""
 import os
 import sys
 
@@ -53,8 +54,31 @@ def multi_update():
     fake_peer_worker.main()
 
 
+def rbm_sample():
+    rows, n, bs = 9, 70, 5
+    rng = torch.tensor([12345, 7], dtype=torch.int32, device=dev)
+    for dt in (torch.float32, torch.bfloat16):
+        p = torch.rand(rows, n, device=dev).to(dt)
+        out = torch.empty_like(p)
+        ext.rbm_sample(p, out, bs, rng)
+        torch.cuda.synchronize()
+        assert torch.equal(out[bs:], p[bs:]) and bool(((out[:bs] == 0) | (out[:bs] == 1)).all())
+
+
+def rbm_apply():
+    h, v = 45, 37
+    w = torch.randn(h, v, device=dev)
+    g = torch.randn(v, h, device=dev)
+    hb, hg, vb, vg = (torch.randn(k, device=dev) for k in (h, h, v, v))
+    want = (w + 0.5 * g.t(), hb + 0.5 * hg, vb + 0.5 * vg)
+    ext.rbm_apply(w, g, hb, hg, vb, vg, 0.5)
+    torch.cuda.synchronize()
+    assert all(torch.allclose(a, b) for a, b in zip((w, hb, vb), want))
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["gemm_single", "conv_umma", "gemm_pair", "multi_update"]
+    which = sys.argv[1:] or ["gemm_single", "conv_umma", "gemm_pair", "multi_update", "rbm_sample",
+                             "rbm_apply"]
     for name in which:
         globals()[name]()
         print("ok", name, flush=True)

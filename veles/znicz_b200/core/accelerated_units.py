@@ -127,13 +127,3 @@ class AcceleratedWorkflow(Workflow):
             device = get_device(device)
         self.device = device
         return super().initialize(device=device, **kwargs)
-
-
-class EmptyDeviceMethodsMixin(object):
-    """Units whose math is host-only (RBM helpers, /root/reference/rbm_units.py:54-68)."""
-
-    def cuda_init(self):
-        pass
-
-    def cuda_run(self):
-        self.numpy_run()

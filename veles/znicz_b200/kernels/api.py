@@ -1049,6 +1049,73 @@ def evaluate_mse(unit):
 
 
 # ------------------------------------------------------------------------------------------
+# restricted Boltzmann machines (ops/rbm_units.py; csrc/rbm.cu)
+# ------------------------------------------------------------------------------------------
+def rbm_sample(unit):
+    """Binarization: Bernoulli(input) on the first batch_size rows, input copied on the rest."""
+    _ext(unit).rbm_sample(unit.input.dev, unit.output.dev_out, int(unit.batch_size), unit.rng_up_.dev)
+    _launch()
+
+
+def _col_mean(unit, ext, name, x, rows, cols, out):
+    """out[1][cols] = mean of the first ``rows`` rows of x: the bias-gradient column sums
+    (ACT_LINEAR: x is only read) per row slice, their sum, and the 1/rows scale."""
+    slices = ext.colsum_slices(rows)
+    parts = _tmp(unit, name + "_parts", (slices, cols), torch.float32)
+    sums = _tmp(unit, name + "_sums", (1, cols), torch.float32)
+    ext.err_act_colsum(x, None, rows, cols, ACT_LINEAR, parts)
+    ext.col_sums(parts, sums, slices, cols, False)
+    ext.axpby_2d(sums, 0, out.dev_out.view(1, cols), 0, cols, 1.0 / rows, 0.0)
+    _launch(3)
+
+
+def rbm_batch_stats(unit):
+    """BatchWeights: weights_batch[V][H] = v^T h / bs, vbias_batch = <v>, hbias_batch = <h> over the
+    first batch_size rows (the GEMM's reduction length is bs, so the rows past it never enter)."""
+    ext = _ext(unit)
+    v, h = unit.v.dev, unit.h.dev
+    bs = int(unit.batch_size)
+    nv, nh = v.numel() // v.shape[0], h.numel() // h.shape[0]
+    wb = unit.weights_batch.dev_out
+    if _is_bf16(v) and _is_bf16(h) and nv % 8 == 0 and nh % 8 == 0:
+        # the FC weight-gradient form: (h^T . v) with a transposed store = v^T . h
+        r = ext.gemm(h, nh, True, v, nv, False, wb, nh, True, nh, nv, bs, None, 0, 1.0 / bs, 0.0,
+                     1, 0, 1)
+        if r != 0:
+            raise RuntimeError("%s: wgmma v^T h refused the shape (code %d)" % (unit, r))
+    else:
+        _path(unit, "rbm_stats:simt")
+        ext.gemm(v, nv, True, h, nh, False, wb, nh, False, nv, nh, bs, None, 0, 1.0 / bs, 0.0,
+                 1, 0, 0)
+    _launch()
+    _col_mean(unit, ext, "v_mean", v, bs, nv, unit.vbias_batch)
+    _col_mean(unit, ext, "h_mean", h, bs, nh, unit.hbias_batch)
+
+
+def rbm_gradients(unit):
+    """GradientsCalculator: grad = positive-phase statistic - negative-phase statistic."""
+    ext = _ext(unit)
+    for g, s0, s1 in ((unit.vbias_grad, unit.vbias0, unit.vbias1),
+                      (unit.hbias_grad, unit.hbias0, unit.hbias1),
+                      (unit.weights_grad, unit.weights0, unit.weights1)):
+        a, b = s0.dev, s1.dev
+        out = g.dev_out
+        n = out.numel() // out.shape[0]
+        ext.axpby_2d(a, 0, out, 0, n, 1.0, 0.0)
+        ext.axpby_2d(b, 0, out, 0, n, -1.0, 1.0)
+        _launch(2)
+
+
+def rbm_apply(unit):
+    """WeightsUpdater: W[h][v] += lr * weights_grad[v][h], biases += lr * their gradients."""
+    _ext(unit).rbm_apply(unit.weights.dev, unit.weights_grad.dev, unit.hbias.dev, unit.hbias_grad.dev,
+                         unit.vbias.dev, unit.vbias_grad.dev, float(unit.learning_rate))
+    for a in (unit.weights, unit.hbias, unit.vbias):
+        a.dev_written()
+    _launch()
+
+
+# ------------------------------------------------------------------------------------------
 # deconvolution (transposed conv = the conv dgrad / fprop / wgrad kernels with swapped roles)
 # ------------------------------------------------------------------------------------------
 def _deconv_geom(u):

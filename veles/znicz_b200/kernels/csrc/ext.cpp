@@ -42,6 +42,8 @@ void launch_evaluate_mse(const void*, const void*, bool, void*, bool, const floa
 void launch_mse_find_closest(const void*, bool, const float*, const int*, const float*, int, int, int, int*, cudaStream_t);
 void launch_fused_update(const TensorDesc&, const float* const*, int, uint32_t* const*, uint32_t*, int, int, cudaStream_t);
 void launch_col_sums(const float*, float*, int, int, int, cudaStream_t);
+void launch_rbm_sample(const void*, void*, long long, long long, const int*, bool, cudaStream_t);
+void launch_rbm_apply(float*, const float*, float*, const float*, float*, const float*, int, int, float, cudaStream_t);
 void launch_lstm_cell_fwd(const float*, const float*, float*, float*, void*, long long, void*, long long, int, int, bool, cudaStream_t);
 void launch_lstm_cell_bwd(const void*, long long, const void*, long long, const float*, const float*, const float*, const float*, float*, void*, int, int, bool, cudaStream_t);
 int fc_small_max_out();
@@ -690,6 +692,31 @@ void col_sums(Tensor w, Tensor out, int64_t rows, int64_t cols, bool transposed)
   zn::launch_col_sums(w.data_ptr<float>(), out.data_ptr<float>(), (int)rows, (int)cols, transposed ? 1 : 0, cur());
   kcheck();
 }
+// RBM Gibbs sample: out = Bernoulli(in) on the first batch_size rows, a copy of in on the rest
+void rbm_sample(Tensor in, Tensor out, int64_t batch_size, Tensor rng) {
+  chk(in, "in"); chk(out, "out"); same_dt(in, out);
+  TORCH_CHECK(in.scalar_type() != torch::kInt32 && in.numel() == out.numel() && in.dim() >= 1, "rbm_sample: operands");
+  TORCH_CHECK(rng.is_cuda() && rng.scalar_type() == torch::kInt32 && rng.numel() >= 2, "rbm_sample: rng");
+  const int64_t rows = in.size(0), cols = rows ? in.numel() / rows : 0;
+  TORCH_CHECK(batch_size >= 0 && batch_size <= rows, "rbm_sample: batch_size out of range");
+  zn::launch_rbm_sample(in.data_ptr(), out.data_ptr(), batch_size * cols, in.numel(), rng.data_ptr<int>(),
+                        is_bf16(in), cur());
+  kcheck();
+}
+// RBM update: w[H][V] += lr * g[V][H]^T, hbias[H] += lr * hgrad, vbias[V] += lr * vgrad (all fp32)
+void rbm_apply(Tensor w, Tensor g, Tensor hbias, Tensor hgrad, Tensor vbias, Tensor vgrad, double lr) {
+  for (const Tensor* t : {&w, &g, &hbias, &hgrad, &vbias, &vgrad}) {
+    chk(*t, "rbm_apply operand");
+    TORCH_CHECK(t->scalar_type() == torch::kFloat32, "rbm_apply: fp32 operands");
+  }
+  TORCH_CHECK(w.dim() == 2, "rbm_apply: w must be [H][V]");
+  const int64_t H = w.size(0), V = w.size(1);
+  TORCH_CHECK(g.numel() == H * V && hbias.numel() == H && hgrad.numel() == H && vbias.numel() == V &&
+              vgrad.numel() == V, "rbm_apply: shapes");
+  zn::launch_rbm_apply(w.data_ptr<float>(), g.data_ptr<float>(), hbias.data_ptr<float>(), hgrad.data_ptr<float>(),
+                       vbias.data_ptr<float>(), vgrad.data_ptr<float>(), (int)H, (int)V, (float)lr, cur());
+  kcheck();
+}
 void refresh_shadows(Tensor w, int64_t rows, int64_t cols, c10::optional<Tensor> lp, int64_t ld,
                      c10::optional<Tensor> lp_conv, int64_t taps, int64_t C, int64_t c_pad, int64_t lp_cpad) {
   zn::launch_refresh_shadows(w.data_ptr<float>(), w.numel(), (int)rows, (int)cols, bptr_or_null(lp), (int)ld,
@@ -1202,6 +1229,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("get_dp_gradient_scale", []() { return (double)zn::get_dp_gradient_scale(); });
   m.def("multi_update_max_tensors", []() { return (int64_t)zn::MU_MAX_TENSORS; }); m.def("multi_update", &multi_update);
   m.def("col_sums", &col_sums); m.def("refresh_shadows", &refresh_shadows);
+  m.def("rbm_sample", &rbm_sample); m.def("rbm_apply", &rbm_apply);
   m.def("lstm_fwd_persist", &lstm_fwd_persist); m.def("lstm_bwd_persist", &lstm_bwd_persist);
   m.def("lstm_state_floats", &lstm_state_floats); m.def("lstm_part_floats", &lstm_part_floats); m.def("lstm_unpack_state", &lstm_unpack_state);
   m.def("lstm_persist_launches", []() { return (int64_t)zn::lstm_persist_launches(); });

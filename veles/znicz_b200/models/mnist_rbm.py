@@ -1,7 +1,9 @@
 """MnistRBM: CD-1 restricted Boltzmann machine (196 visible, 1000 hidden).
 Parity: /root/reference/tests/research/MnistRBM/mnist_rbm.py:60-186, config :43-51.
 The reference loads 240 14x14 patches from a .mat file; offline the loader falls back to
-down-sampled synthetic digits when ``data_path`` does not exist."""
+down-sampled synthetic digits when ``data_path`` does not exist. Unlike the reference the loader
+is not forced onto the host: on CUDA it gathers the minibatch on the device in the compute
+type's dtype, which the Binarization output and the reconstruction evaluator then share."""
 from __future__ import annotations
 
 import os
@@ -23,7 +25,7 @@ root.mnist_rbm.update({
     "snapshotter": {"prefix": "mnist_rbm"},
     "learning_rate": 0.001,
     "cd_k": 1,
-    "loader": {"minibatch_size": 128, "force_numpy": True,
+    "loader": {"minibatch_size": 128, "force_numpy": False,
                "data_path": os.path.join(str(root.common.dirs.datasets), "rbm_data",
                                          "test_rbm_functional.mat")}})
 

@@ -2,9 +2,15 @@
 
 Parity: /root/reference/rbm_units.py (Binarization :72, IterationCounter :155,
 BatchWeights :182, GradientsCalculator :261, WeightsUpdater :338, MemCpy :366,
-GradientRBM :441 — CD-k Gibbs chain as a nested workflow, EvaluatorRBM :518). As in the
-reference all statistics are host numpy (``EmptyDeviceMethodsMixin`` :54-68); only the
-All2AllSigmoid gates and MemCpy touch the device.
+GradientRBM :441 — CD-k Gibbs chain as a nested workflow, EvaluatorRBM :518). The numpy
+paths are the reference's host statistics (``EmptyDeviceMethodsMixin`` :54-68 ran them on
+the host in every backend).
+
+H100: the whole CD-k step stays on the device. Binarization draws from a counter-based hash
+of (seed, counter, element) (csrc/rbm.cu; ``binarize_twin`` is its exact numpy twin), the
+batch statistics run on the GEMM and column-sum kernels, GradientsCalculator on ``axpby_2d``
+and WeightsUpdater is one launch (``rbm_apply_k``), after which the forward units that read
+the updated weights through a bf16 / fp8 copy rebuild it.
 """
 from __future__ import annotations
 
@@ -16,26 +22,44 @@ from ..core.memory import Array
 from ..core.mutable import Bool
 from ..core.normalization import NoneNormalizer
 from ..core.units import Unit
-from ..core.workflow import Repeater
+from ..core.workflow import Repeater, Workflow
 from ..workflow.evaluator import EvaluatorMSE
 from .all2all import All2AllSigmoid
+from .nn_units import Forward
+from .pooling import hash_u32
 
 
-class HostOnlyMixin(object):
-    """Units whose maths runs on the host in every backend."""
+def binarize_twin(p, batch_size, seed, counter):
+    """The device sampler's rule in numpy: for flat index i of the first ``batch_size`` rows,
+    1 when (hash_u32(seed, counter, i) >> 8) * 2^-24 < p[i] (p as fp32), else 0; the other
+    rows are copied."""
+    p = numpy.asarray(p, dtype=numpy.float32)
+    out = p.copy()
+    n = int(batch_size) * (p.size // p.shape[0])
+    u = (hash_u32(seed, counter, numpy.arange(n, dtype=numpy.uint64)) >> numpy.uint32(8)).astype(
+        numpy.float32) * numpy.float32(2.0 ** -24)
+    out.reshape(-1)[:n] = (u < p.reshape(-1)[:n]).astype(numpy.float32)
+    return out
 
-    def cuda_run(self):
-        self.numpy_run()
 
+class Binarization(AcceleratedUnit):
+    """output(i, j) = 1 with probability input(i, j), else 0 (first batch_size rows).
 
-class Binarization(HostOnlyMixin, AcceleratedUnit):
-    """output(i, j) = 1 with probability input(i, j), else 0 (first batch_size rows)."""
+    numpy: ``matlab_binornd`` on ``rand``. CUDA: the hash sampler of ``binarize_twin``, with a
+    ``seed`` drawn from ``rand`` at initialize and a ``rng_counter`` that advances once per run;
+    both are pickled, so a workflow restored from a snapshot continues the same sample stream."""
 
     def __init__(self, workflow, **kwargs):
         super().__init__(workflow, **kwargs)
         self.output = Array()
         self.rand = kwargs.get("rand", prng.get())
+        self.seed = kwargs.get("seed")
+        self.rng_counter = 0
         self.demand("input", "batch_size")
+
+    def init_unpickled(self):
+        super().init_unpickled()
+        self.rng_up_ = None
 
     def initialize(self, device=None, **kwargs):
         if not self.input:
@@ -43,6 +67,11 @@ class Binarization(HostOnlyMixin, AcceleratedUnit):
         super().initialize(device=device, **kwargs)
         if not self.output or self.output.shape != self.input.shape:
             self.output.reset(numpy.zeros_like(self.input.mem))
+        # 0 / 1 are exact in bf16: a bf16 sample keeps the next GEMM on the tensor cores (and the
+        # device copy a consumer makes of a host sample matches the device units around it)
+        self.output.dev_dtype = self.input.dev_dtype
+        if self.on_cuda and self.seed is None:
+            self.seed = int(self.rand.randint(1, 2 ** 31 - 1))
         self.init_vectors(self.input, self.output)
         return None
 
@@ -58,6 +87,18 @@ class Binarization(HostOnlyMixin, AcceleratedUnit):
         bs = int(self.batch_size)
         self.output.mem[...] = self.input.mem
         self.output.mem[:bs] = self.matlab_binornd(1, self.input.mem[:bs])
+
+    def cuda_prepare(self):
+        if self.rng_up_ is None:
+            import torch
+            from ..core.memory import ScalarUploader
+            self.rng_up_ = ScalarUploader(self.device, 2, torch.int32)
+        self.rng_up_.upload((self.seed & 0x7FFFFFFF, self.rng_counter & 0x7FFFFFFF))
+        self.rng_counter += 1
+
+    def cuda_run(self):
+        from ..kernels import api
+        api.rbm_sample(self)
 
 
 class BinarizationGradH(Binarization):
@@ -93,7 +134,7 @@ class IterationCounter(Unit):
         self.complete <<= self.iteration > self.max_iterations
 
 
-class BatchWeights(HostOnlyMixin, AcceleratedUnit):
+class BatchWeights(AcceleratedUnit):
     """<v hᵀ>, <v>, <h> over the minibatch."""
 
     def __init__(self, workflow, **kwargs):
@@ -115,6 +156,7 @@ class BatchWeights(HostOnlyMixin, AcceleratedUnit):
             self.vbias_batch.reset(numpy.zeros((1, vsz), dtype=self.h.dtype))
         if not self.weights_batch:
             self.weights_batch.reset(numpy.zeros((vsz, hsz), dtype=self.h.dtype))
+        self.init_vectors(self.weights_batch, self.hbias_batch, self.vbias_batch)
         return None
 
     def numpy_run(self):
@@ -129,12 +171,16 @@ class BatchWeights(HostOnlyMixin, AcceleratedUnit):
         self.vbias_batch.mem[...] = v.sum(axis=0, keepdims=True) / bs
         self.hbias_batch.mem[...] = h.sum(axis=0, keepdims=True) / bs
 
+    def cuda_run(self):
+        from ..kernels import api
+        api.rbm_batch_stats(self)
+
 
 class BatchWeights2(BatchWeights):
     pass
 
 
-class GradientsCalculator(HostOnlyMixin, AcceleratedUnit):
+class GradientsCalculator(AcceleratedUnit):
     """grad = positive-phase statistics − negative-phase statistics."""
 
     def __init__(self, workflow, **kwargs):
@@ -152,6 +198,7 @@ class GradientsCalculator(HostOnlyMixin, AcceleratedUnit):
                        (self.weights_grad, self.weights0)):
             if not g or g.shape != ref.shape:
                 g.reset(numpy.zeros(ref.shape, dtype=ref.dtype))
+        self.init_vectors(self.hbias_grad, self.vbias_grad, self.weights_grad)
         return None
 
     def numpy_run(self):
@@ -164,19 +211,51 @@ class GradientsCalculator(HostOnlyMixin, AcceleratedUnit):
         self.hbias_grad.mem[...] = self.hbias0.mem - self.hbias1.mem
         self.weights_grad.mem[...] = self.weights0.mem - self.weights1.mem
 
+    def cuda_run(self):
+        from ..kernels import api
+        api.rbm_gradients(self)
 
-class WeightsUpdater(Unit):
-    """weights += lr · gradᵀ; biases += lr · grad."""
+
+def _all_units(workflow):
+    for u in workflow:
+        yield u
+        if isinstance(u, Workflow):
+            yield from _all_units(u)
+
+
+class WeightsUpdater(AcceleratedUnit):
+    """weights += lr · gradᵀ; biases += lr · grad.
+
+    The forward units that read ``weights`` (in mnist_rbm the hidden layer and the Gibbs chain's
+    make_h) keep bf16 / fp8 copies of it on the device: each run rebuilds them."""
 
     def __init__(self, workflow, **kwargs):
         super().__init__(workflow, **kwargs)
         self.learning_rate = kwargs["learning_rate"]
         self.demand("hbias_grad", "vbias_grad", "weights_grad", "weights", "hbias", "vbias")
 
-    def initialize(self, **kwargs):
-        pass
+    def init_unpickled(self):
+        super().init_unpickled()
+        self.readers_ = []
+
+    def initialize(self, device=None, **kwargs):
+        super().initialize(device=device, **kwargs)
+        if self.on_cuda:
+            self.init_vectors(self.hbias_grad, self.vbias_grad, self.weights_grad, self.weights,
+                              self.hbias, self.vbias)
+        self.readers_ = [u for u in _all_units(self.workflow)
+                         if isinstance(u, Forward) and u.weights is self.weights]
+        return None
 
     def run(self):
+        if self._backend_run_ is None:
+            self.initialize()      # run without initialize(): the host update
+        super().run()
+        for fwd in self.readers_:
+            if fwd.on_cuda:
+                fwd.refresh_shadows()
+
+    def numpy_run(self):
         for a in (self.hbias_grad, self.vbias_grad, self.weights_grad):
             a.map_read()
         for a in (self.weights, self.hbias, self.vbias):
@@ -186,6 +265,10 @@ class WeightsUpdater(Unit):
         self.vbias.mem += self.learning_rate * self.vbias_grad.mem.reshape(self.vbias.shape)
         for a in (self.weights, self.hbias, self.vbias):
             a.unmap()
+
+    def cuda_run(self):
+        from ..kernels import api
+        api.rbm_apply(self)
 
 
 class MemCpy(AcceleratedUnit):
