@@ -3,7 +3,8 @@ hand-rolled synchronisation protocol of the repo on sizes a sanitizer run can fi
 gemm_umma_k (mbarrier ring, TMA + LDGSTS producers, wgmma), gemm_pair_k (producer / MMA
 warpgroups, TMA-store epilogue), lstm kernels (barrier.cluster), multi_update_k (grid barrier;
 fake-peer flag protocol with 2 ranks sharing the GPU), fc_small, pooling / LRN / evaluator,
-rbm_sample_k / rbm_apply_k (ragged shapes: partial batch, partial transpose tiles)."""
+rbm_sample_k / rbm_apply_k (ragged shapes: partial batch, partial transpose tiles),
+render_shots_k (1 x N and N x 1 pictures, boxes over the edges, rows past n, padded copy)."""
 import os
 import sys
 
@@ -76,9 +77,38 @@ def rbm_apply():
     assert all(torch.allclose(a, b) for a, b in zip((w, hb, vb), want))
 
 
+def render_shots():
+    import numpy
+    from veles.znicz_b200.models.imagenet_forward.loader import shot_table_row
+    a, c, rows = 13, 3, 7
+    pics = [(1, 30), (25, 1), (17, 22)]               # h, w: 1 x N, N x 1 and a plain picture
+    arena = torch.randint(0, 256, (sum(h * w * c for h, w in pics) + 5,), dtype=torch.uint8,
+                          device=dev)
+    table = numpy.zeros((rows, 8))
+    geo = numpy.zeros((rows, 4), numpy.int64)
+    at = 5
+    for r, (h, w) in enumerate(pics * 2):
+        if r < len(pics):
+            geo[r] = (at, h, w, r % 2)
+            at += h * w * c
+        else:
+            geo[r] = geo[r - len(pics)]
+        box = {"x": w - 1.0, "y": 0.0, "width": 9.0 + r, "height": 8.0}
+        table[r] = shot_table_row(box, 0.7 * r - 2.0, a)
+    hdr = torch.tensor([rows - 2, 0, 0, 0], dtype=torch.int32, device=dev)
+    mean = torch.rand(a, a, c, device=dev)
+    for dt in (torch.float32, torch.bfloat16):
+        out = torch.empty(rows, a, a, c, device=dev, dtype=dt)
+        pad = torch.empty(rows, a, a, 8, device=dev, dtype=dt)
+        ext.render_shots(arena, hdr, torch.from_numpy(table).to(dev), torch.from_numpy(geo).to(dev),
+                         mean, out, pad)
+        torch.cuda.synchronize()
+        assert not out[rows - 2:].any() and torch.equal(pad[..., :c], out) and not pad[..., c:].any()
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["gemm_single", "conv_umma", "gemm_pair", "multi_update", "rbm_sample",
-                             "rbm_apply"]
+                             "rbm_apply", "render_shots"]
     for name in which:
         globals()[name]()
         print("ok", name, flush=True)

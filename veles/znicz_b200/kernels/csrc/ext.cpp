@@ -56,6 +56,8 @@ long long conv_pair_launches();
 long long conv_halo_launches();
 long long augment_launches();
 void launch_augment_minibatch(const uint8_t*, long long, const int*, const int*, const int*, const float*, void*, void*, bool, const int*, int*, int, int, int, int, int, int, cudaStream_t);
+long long render_shots_launches();
+void launch_render_shots(const uint8_t*, long long, const int*, const double*, const long long*, const float*, void*, void*, bool, int, int, int, cudaStream_t);
 int launch_fc_wgrad_pair(const void*, long long, const void*, long long, float*, long long, int, int, int,
                          cudaStream_t);
 void set_dp_gradient_scale(float);
@@ -262,6 +264,46 @@ void augment_minibatch(Tensor src, Tensor hdr, c10::optional<Tensor> idx, Tensor
                                params.data_ptr<int>(), mp, dst.data_ptr(), pad, is_bf16(dst),
                                has_ls ? labels_src->data_ptr<int>() : nullptr,
                                has_ld ? labels_dst->data_ptr<int>() : nullptr, max_rows, sy, sx, C, cy, cx, cur());
+  kcheck();
+}
+// Localisation shots (csrc/render.cu): row r < hdr[0] renders the uint8 picture [h][w][C] at byte
+// offset pics[r] = (off, h, w, flip) of arena with shots[r] = (ca, sa, scale, bw/2, bh/2, cx, cy, -);
+// rows >= hdr[0] are zero.
+void render_shots(Tensor arena, Tensor hdr, Tensor shots, Tensor pics, c10::optional<Tensor> mean,
+                  Tensor dst, c10::optional<Tensor> dst_pad) {
+  auto dev_tensor = [](const Tensor& t, const char* name, c10::ScalarType dt) {
+    TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.scalar_type() == dt, "render_shots: ", name,
+                " must be a contiguous ", c10::toString(dt), " CUDA tensor");
+  };
+  dev_tensor(arena, "arena", torch::kUInt8);
+  chk(dst, "dst");
+  TORCH_CHECK((dst.scalar_type() == torch::kFloat32 || is_bf16(dst)) && dst.dim() == 4 && dst.size(1) == dst.size(2),
+              "render_shots: dst must be fp32 or bf16 [n][A][A][C]");
+  const int max_rows = (int)dst.size(0), A = (int)dst.size(1), C = (int)dst.size(3);
+  TORCH_CHECK(max_rows >= 1 && max_rows <= 65535 && A >= 1 && C >= 1 && C <= 8,
+              "render_shots: needs 1..65535 rows and 1..8 channels, got ", max_rows, " and ", C);
+  dev_tensor(hdr, "hdr", torch::kInt32);
+  dev_tensor(shots, "shots", torch::kFloat64);
+  dev_tensor(pics, "pics", torch::kInt64);
+  TORCH_CHECK(hdr.numel() >= 1, "hdr must hold n");
+  TORCH_CHECK(shots.numel() == 8LL * max_rows, "shots must be float64 [n][8]");
+  TORCH_CHECK(pics.numel() == 4LL * max_rows, "pics must be int64 [n][4]");
+  const float* mp = nullptr;
+  if (mean.has_value() && mean->defined()) {
+    chk(*mean, "mean");
+    TORCH_CHECK(mean->scalar_type() == torch::kFloat32 && mean->numel() == (int64_t)A * A * C,
+                "mean must be fp32 [A][A][C]");
+    mp = mean->data_ptr<float>();
+  }
+  void* pad = nullptr;
+  if (dst_pad.has_value() && dst_pad->defined()) {
+    chk(*dst_pad, "dst_pad"); same_dt(dst, *dst_pad);
+    TORCH_CHECK(C < 8 && dst_pad->numel() == (int64_t)max_rows * A * A * 8, "padded minibatch must be [n][A][A][8]");
+    pad = dst_pad->data_ptr();
+  }
+  zn::launch_render_shots(arena.data_ptr<uint8_t>(), arena.numel(), hdr.data_ptr<int>(), shots.data_ptr<double>(),
+                          (const long long*)pics.data_ptr<int64_t>(), mp, dst.data_ptr(), pad, is_bf16(dst),
+                          max_rows, A, C, cur());
   kcheck();
 }
 // dst (device) <- src (pinned host tensor), by a kernel that reads the host memory (see
@@ -1205,6 +1247,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gather_minibatch", &gather_minibatch);
   m.def("augment_minibatch", &augment_minibatch);
   m.def("augment_launches", []() { return (int64_t)zn::augment_launches(); });
+  m.def("render_shots", &render_shots);
+  m.def("render_shots_launches", []() { return (int64_t)zn::render_shots_launches(); });
   m.def("swap01_2d", &swap01_2d); m.def("device_copy", &device_copy); m.def("metric_reduce", &metric_reduce);
   m.def("space_to_depth", &space_to_depth); m.def("s2d_pack_weights", &s2d_pack_weights); m.def("s2d_unpack_grad", &s2d_unpack_grad);
   m.def("stream_ring_create", &stream_ring_create); m.def("stream_ring_destroy", &stream_ring_destroy);

@@ -88,6 +88,9 @@ class ImagenetForward(AcceleratedWorkflow):
         shape[0] = self.loader.max_minibatch_size
         self.loader.entry_shape = shape
         self.loader.mean = mean
+        # a bf16 first layer takes its input in bf16 (the wgmma path); the normaliser computes
+        # in fp32, so in front of it the minibatch stays fp32
+        self.loader.feeds_first_layer = normalizer is None
         first = self.forwards[0]
         if normalizer is not None:
             normalizer.workflow = self
